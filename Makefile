@@ -1,15 +1,15 @@
-# Convenience targets; the driver uses __graft_entry__.py / pytest / bench.py directly.
+# Convenience targets over __graft_entry__.py / pytest / bench.py.
 PY ?= python
 
 .PHONY: build test test-gpu bench bench-ref stress clean
 
-build:            ## libbsgpu.so (nvcc, sm_100a) + the CPU oracle; no GPU needed
+build:            ## libbsgpu.so (nvcc, sm_90a) + the CPU oracle; no GPU needed
 	$(PY) __graft_entry__.py
 
 test: build       ## CPU suite: oracle vs the reference's fixtures, ABI, layout models, gloo sharding
 	$(PY) -m pytest tests -x -q -m "not gpu"
 
-test-gpu: build   ## parity tests through the C ABI (needs a B200)
+test-gpu: build   ## parity tests through the C ABI (needs an H100)
 	$(PY) -m pytest tests -x -q -m gpu
 
 bench: build      ## headline benchmark, one GPU

@@ -2,12 +2,12 @@
 """bench.py -- headline benchmark of the packed-genotype hot path (BASELINE.json metric:
 "genotypes/sec in bed_prodVec").
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload cfg2|cfg5]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload cfg2|cfg5] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A step is one bed_prodVec (X~ . y, binomial center/scale, all rows, all columns) over the resident synthetic
 .bed.  Workload (default, `cfg5`) = BASELINE.json configs[4], the matrix the metric is quoted on: UKBB-shaped
-487,000 samples x 1,100,000 SNPs (134 GB packed, SNP-major copy only: it fits one 180 GB GPU), SNP columns split
+487,000 samples x 500,000 SNPs (60.9 GB packed, SNP-major copy only: it fits one 80 GB H100), SNP columns split
 over the N ranks (STRONG scaling), every step ending in one all-reduce of the n-vector of partial products; the
 same line carries the second headline, bed_randomSVD(k = 20) wall time.  `--workload cfg2` is configs[1]
 (50,000 x 500,000 per GPU, weak scaling, SVD k = 10); at N = 1 the default run appends it as `extra.cfg2`.
@@ -42,8 +42,8 @@ SEED = 20250924 + 1  # SURVEY.md section 8d: 20250924 + config index
 WORKLOADS = {
     "cfg2": dict(n=50_000, m=500_000, scaling="weak", svd_k=10,
                  name="configs[1]: bed_prodVec on synthetic 50,000 x 500,000 2-bit .bed per GPU (binomial center/scale)"),
-    "cfg5": dict(n=487_000, m=1_100_000, scaling="strong", svd_k=20,
-                 name="configs[4]: bed_prodVec on UKBB-shaped synthetic 487,000 x 1,100,000 .bed, SNP columns sharded over the GPUs"),
+    "cfg5": dict(n=487_000, m=500_000, scaling="strong", svd_k=20,
+                 name="configs[4]: bed_prodVec on UKBB-shaped synthetic 487,000 x 500,000 .bed, SNP columns sharded over the GPUs"),
 }
 
 
@@ -54,7 +54,7 @@ def measured_peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet HBM3 bandwidth (3.35 TB/s), not a measurement"
 
 
 class ClockSampler(threading.Thread):
@@ -230,21 +230,6 @@ def run_reference(args, wl):
     return 0
 
 
-def traffic_for(kernel, alg_bytes):
-    """DRAM bytes per launch of the dominant kernel: the ratio (dram read + write) / algorithmic bytes measured by the
-    committed ncu --set full captures of the same kernel (bench.py cannot run under ncu and report a number), applied to
-    this launch's algorithmic bytes; the source file is named beside the value."""
-    tp = os.path.join(ROOT, "profiles", "r02_pmv_traffic.json")
-    try:
-        d = json.load(open(tp))
-        r = d["ratio_vs_algorithmic"].get(kernel)
-        if r:
-            return float(r) * alg_bytes, "profiles/r02_pmv_traffic.json: measured ratio %.4f x algorithmic bytes; %s" % (r, d["source"])
-    except Exception:
-        pass
-    return None, None
-
-
 def run_workload(args, wl_key, torch, dist, B, L, rank, world, local, with_cpu, layout):
     """One workload on this process group: timed products, roofline, e2e (pinned and pageable host buffers), parity
     against the oracle on a bounded sample, bed_randomSVD wall time.  Returns the JSON pieces (rank 0) or None."""
@@ -311,6 +296,10 @@ def run_workload(args, wl_key, torch, dist, B, L, rank, world, local, with_cpu, 
         dist.barrier()
     clocks = sampler.stop()
     ms = ev0.elapsed_time(ev1)
+    if args.dump_outputs and rank == 0:
+        # what the last timed step returned: the n-vector X~.y (summed over the ranks), same inputs on every run
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "%s_prodvec.npy" % wl_key), out.cpu().numpy().astype(np.float64))
     launches = int(L.bsg_launch_count() - launches0)
     cnt, tot = C.c_int(0), C.c_double(0)
     _lib.check(L.bsg_kernel_time_stats(C.byref(cnt), C.byref(tot)))
@@ -334,9 +323,8 @@ def run_workload(args, wl_key, torch, dist, B, L, rank, world, local, with_cpu, 
     # with missing values the product kernel runs in its no-missing mode and bsg::naell::k_corr adds the list sums
     # (bigsnpr_b200/csrc/bsg_naell.cu); kernel_ms is the product kernel alone, ms_per_step the whole step
     kernel = "bsg::pmv::k_pmv" if (layouts & 2) else "bsg::pmvt::k_pmvT"
-    traffic, traffic_src = traffic_for(kernel, alg_bytes)
     roofline = {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                "frac": (achieved / peak) if achieved else None, "traffic": traffic, "traffic_source": traffic_src,
+                "frac": (achieved / peak) if achieved else None,
                 "kernel": kernel, "kernel_ms": kern_ms, "launches_timed": cnt.value,
                 "algorithmic_bytes_per_launch": alg_bytes, "peak_source": peak_src,
                 "kernel_share_of_step": (kern_ms * args.steps / ms) if ms > 0 else None}
@@ -497,7 +485,7 @@ def run_workload(args, wl_key, torch, dist, B, L, rank, world, local, with_cpu, 
         "value": value, "ms_per_step": ms / args.steps, "scaling": wl["scaling"],
         "config": {"workload": wl["name"], "n": n, "m_total": m_total, "m_per_gpu": m_loc, "na_rate": args.na_rate,
                    "layouts": layouts,
-                   "l2": "inputs larger than L2: %.2f GB of packed genotypes per pass per GPU vs 126 MB L2" % (alg_bytes / 1e9),
+                   "l2": "inputs larger than L2: %.2f GB of packed genotypes per pass per GPU vs 50 MB L2" % (alg_bytes / 1e9),
                    "arithmetic": "exact int8 x uint2 on the integer tensor pipe, 61-bit fixed-point vector, fp64 epilogue",
                    "parallelism": par},
         "roofline": roofline, "cpu_baseline": cpu_baseline, "parity": parity,
@@ -526,10 +514,12 @@ def main():
     ap.add_argument("--no-extra", action="store_true", help="skip the configs[1] extra leg of the default N = 1 run")
     ap.add_argument("--layout", choices=("auto", "both", "snp"), default="auto",
                     help="snp: the SNP-major copy only (the library's default; X.y on k_pmvT); both: also the sample-major "
-                         "copy (X.y on k_pmv); auto: snp for cfg5 (134 GB), both for cfg2")
+                         "copy (X.y on k_pmv); auto: snp for cfg5 (60.9 GB), both for cfg2")
     ap.add_argument("--nccl", action="store_true", help="N > 1: reduce with torch.distributed / NCCL instead of the library's "
                                                        "own peer-memory communicator (the baseline it is measured against)")
     ap.add_argument("--no-single-copy", action="store_true", help="skip the extra leg timing X.y on the SNP-major copy alone")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the result of the last step as DIR/<workload>_prodvec.npy (float64)")
     args = ap.parse_args()
     wl = WORKLOADS[args.workload]
     if args.impl == "reference":
@@ -556,10 +546,10 @@ def main():
     import bigsnpr_b200 as B
     from bigsnpr_b200 import _lib, build
 
-    if rank == 0:
-        build.build()
-    if world > 1:
-        dist.barrier()
+    # the benchmark compiles nothing (its tree may be read-only), but it refuses to time a library older than its sources
+    if build.stale():
+        raise SystemExit("bigsnpr_b200/libbsgpu.so is missing or older than its sources: "
+                         "run python -m bigsnpr_b200.build first")
     L = _lib.lib()
     dev = torch.device("cuda", local)
     # a dedicated (non-default) stream: the library enqueues on the stream it is handed, and the CUDA events that time

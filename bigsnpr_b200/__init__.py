@@ -1,4 +1,4 @@
-"""bigsnpr_b200 -- B200-native (sm_100a) engine for bigsnpr's packed-genotype hot path.
+"""bigsnpr_b200 -- H100-native (sm_90a) engine for bigsnpr's packed-genotype hot path.
 
 The product is the C-ABI CUDA library ``libbsgpu.so`` (include/bsgpu.h).  This package is its Python host
 side: a mirror of the reference's R functions (``api``), the loader (``_lib``) and the in-tree build

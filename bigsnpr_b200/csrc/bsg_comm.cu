@@ -194,7 +194,7 @@ static ArArgs ar_args(bsg_comm *c) {
 }
 
 static int ar_grid(int64_t len, int device) {
-  int nsm = 148;
+  int nsm = 132;
   cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, device);
   return (int)std::max<int64_t>(1, std::min<int64_t>((len + 255) / 256, 2 * nsm));  // <= one resident wave
 }
@@ -242,7 +242,7 @@ static int comm_allreduce_twoshot(bsg_comm *c, double *const *bufs, int64_t coun
   a.world = c->world;
   a.rank = c->rank;
   for (int q = 0; q < c->world; q++) a.buf[q] = bufs[q];
-  const int grid = 4 * 148;
+  const int grid = 4 * 132;
   BSG_TRY(comm_barrier(c, s));  // every partial is complete
   k_ar2_reduce<<<grid, 256, 0, s>>>(a, count);
   BSG_TRY(comm_barrier(c, s));  // every slice is reduced
@@ -667,7 +667,7 @@ int bsg_group_randomsvd(bsg_group *g, const int *ind_row, int nr, const int *ind
 }
 
 // bed_tcrossprodSelf over the shards: K = sum_g X~_g X~_g^T.  One host thread per device runs the shard's Gram product
-// (tcgen05 tiles, bsg_la.cu) into a device buffer; the partials are summed in place by the two-shot all-reduce over
+// (wgmma tiles, bsg_la.cu) into a device buffer; the partials are summed in place by the two-shot all-reduce over
 // peer memory and the first device's copy goes back to the host.
 int bsg_group_tcrossprod(bsg_group *g, const int *ind_row, int nr, const int *ind_col, int nc, const double *center,
                          const double *scale, double *K) {

@@ -86,7 +86,7 @@ int compact_lines(const uint8_t *src, int64_t src_stride, const int *code_idx, i
                   int nlines, uint8_t *out, int64_t out_stride, cudaStream_t s) {
   if (nlines == 0) return BSG_OK;
   int64_t work = (int64_t)nlines * (out_stride / 4);
-  k_compact<<<(int)std::min<int64_t>((work + 255) / 256, 148 * 32), 256, 0, s>>>(src, src_stride, code_idx, ncodes, line_idx,
+  k_compact<<<(int)std::min<int64_t>((work + 255) / 256, 132 * 32), 256, 0, s>>>(src, src_stride, code_idx, ncodes, line_idx,
                                                                                nlines, out, out_stride);
   count_launch();
   BSG_CUDA(cudaGetLastError());
@@ -95,7 +95,7 @@ int compact_lines(const uint8_t *src, int64_t src_stride, const int *code_idx, i
 
 int line_counts(const uint8_t *P, int64_t stride, int nlines, int L, int32_t *cnt, uint8_t *na, cudaStream_t s) {
   if (nlines == 0) return BSG_OK;
-  k_line_counts_ext<<<(int)std::min<int64_t>(((int64_t)nlines * 32 + 255) / 256, 148 * 32), 256, 0, s>>>(P, stride, nlines, L,
+  k_line_counts_ext<<<(int)std::min<int64_t>(((int64_t)nlines * 32 + 255) / 256, 132 * 32), 256, 0, s>>>(P, stride, nlines, L,
                                                                                                        cnt, na);
   count_launch();
   BSG_CUDA(cudaGetLastError());
@@ -565,7 +565,7 @@ static int cor_common(bsg_bed *h, const int *ind_row, int nr, const int *ind_col
     BSG_CUDA(cudaMalloc((void **)&sc.M, (size_t)stride * (nc > 0 ? nc : 1)));
     if (nc > 0) {
       int64_t work = (int64_t)nc * (stride / 4);
-      int grid = (int)std::min<int64_t>((work + 255) / 256, 148 * 32);
+      int grid = (int)std::min<int64_t>((work + 255) / 256, 132 * 32);
       k_compact<<<grid, 256, 0, s>>>(h->A, h->strideA, d_row, nr, d_col, nc, sc.M, stride);
       count_launch();
     }
@@ -616,7 +616,7 @@ static int cor_common(bsg_bed *h, const int *ind_row, int nr, const int *ind_col
       }
     } gd{d_cnt, d_na, nullptr, nullptr, nullptr};
     {
-      int grid = (int)std::min<int64_t>(((int64_t)nc * 32 + 255) / 256, 148 * 32);
+      int grid = (int)std::min<int64_t>(((int64_t)nc * 32 + 255) / 256, 132 * 32);
       k_line_counts_ext<<<grid, 256, 0, s>>>(sc.M, stride, nc, nr, d_cnt, d_na);
       count_launch();
     }
@@ -626,7 +626,7 @@ static int cor_common(bsg_bed *h, const int *ind_row, int nr, const int *ind_col
     const int nchunks = (int)(stride / CHUNK);
     const int npad = nchunks * 256 - nr;  // code-0 slots beyond the last row count as valid on both sides
     const int nib = (nc + TM - 1) / TM;
-    // no missing value at all -> 128 x 128 tiles on tcgen05 (bsg_gram5.cu); else 128 x 64 six-plane IMMA tiles
+    // no missing value at all -> 128 x 128 wgmma tiles (bsg_gram5.cu); else 128 x 64 six-plane IMMA tiles
     bool clean = true;
     for (int j = 0; j < nc && clean; j++) clean = na[j] == 0;
     static int use_g5 = -1;
@@ -634,7 +634,7 @@ static int cor_common(bsg_bed *h, const int *ind_row, int nr, const int *ind_col
       const char *ev = getenv("BSG_GRAM5");
       use_g5 = (ev && ev[0] == '0') ? 0 : 1;
     }
-    const bool g5 = use_g5 != 0;  // tcgen05 tiles (128 x 128): missing-free tiles one product, the others six planes
+    const bool g5 = use_g5 != 0;  // wgmma tiles (128 x 128): missing-free tiles one product, the others six planes
     (void)clean;
     const int TNv = g5 ? 128 : TN;
     // any-missing flag per column block
@@ -692,7 +692,7 @@ static int cor_common(bsg_bed *h, const int *ind_row, int nr, const int *ind_col
       if (g5) {
         bool any0 = false, any1 = false;
         for (const Tile &tl : tiles) (tl.mode ? any1 : any0) = true;
-        // TMA-fed 2-CTA tiles over operands expanded once (bsg_gramt.cu); in-kernel expansion when they do not fit
+        // TMA-fed wgmma tiles over operands expanded once (bsg_gramt.cu); in-kernel expansion when they do not fit
         bool done = false;
         int rc5 = gramt_enabled() ? gramt_cor(sc.M, stride, nc, tiles.data(), (int)tiles.size(), d_sums, h->device, s, &done) : BSG_OK;
         if (!rc5 && !done) rc5 = gram5_launch(sc.M, stride, nc, stride, d_tiles, (int)tiles.size(), d_sums, any0, any1, s);
@@ -706,7 +706,7 @@ static int cor_common(bsg_bed *h, const int *ind_row, int nr, const int *ind_col
         k_gram<<<(unsigned)tiles.size(), THREADS, 0, s>>>(sc.M, stride, nc, nchunks, d_tiles, d_sums);
       }
       const long long npairs = w.boff[j0_end] - w.boff[j0_begin];
-      const int eg = (int)std::min<long long>((npairs + 255) / 256, 148 * 16);
+      const int eg = (int)std::min<long long>((npairs + 255) / 256, 132 * 16);
       if (clump && clump->fbm)
         k_cor_from_sums<3><<<eg, 256, 0, s>>>(d_sums, d_tiles, d_rbs, ib_start, j0_begin, j0_end, sc.wlen, sc.boff, d_cnt, nr,
                                               npad, nullptr, nullptr, sc.keep, TNv, d_cc, d_cs, clump->thr);
@@ -763,7 +763,7 @@ int bsg_cor(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, int nc, 
     }
   } g2{d_cnt, d_p, nullptr, nullptr};
   if (nc > 0) {
-    k_count_keep<<<(int)std::min<int64_t>(((int64_t)nc * 32 + 255) / 256, 148 * 16), 256, 0, s>>>(sc.keep, sc.boff, sc.wlen, nc,
+    k_count_keep<<<(int)std::min<int64_t>(((int64_t)nc * 32 + 255) / 256, 132 * 16), 256, 0, s>>>(sc.keep, sc.boff, sc.wlen, nc,
                                                                                                fill_diag, d_cnt);
     count_launch();
   }
@@ -794,7 +794,7 @@ int bsg_cor(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, int nc, 
     g2.d = d_ox;
     if (e == cudaSuccess) e = cudaMemcpyAsync(d_p, hp.data(), (size_t)(nc + 1) * sizeof(long long), cudaMemcpyHostToDevice, s);
     if (e == cudaSuccess) {
-      k_fill_csc<<<(int)std::min<int64_t>(((int64_t)nc * 32 + 255) / 256, 148 * 16), 256, 0, s>>>(
+      k_fill_csc<<<(int)std::min<int64_t>(((int64_t)nc * 32 + 255) / 256, 132 * 16), 256, 0, s>>>(
           sc.band, sc.keep, sc.boff, sc.wlen, d_p, nc, fill_diag, d_oi, d_ox);
       count_launch();
       // The result arrays are fresh malloc memory (configs[2]: 1.2 GB): first touch by one thread runs at ~1.5 GB/s and
@@ -953,7 +953,7 @@ static int clumping_common(bsg_bed *h, const int *ind_row, int nr, const int *in
     BSG_CUDA(cudaMemcpyAsync(d_rank, rank.data(), (size_t)nc * sizeof(int), cudaMemcpyHostToDevice, s));
     BSG_CUDA(cudaMemcpyAsync(d_pos, pos, (size_t)nc * sizeof(double), cudaMemcpyHostToDevice, s));
     BSG_CUDA(cudaMemsetAsync(d_state, 0xFF, (size_t)nc * sizeof(int), s));  // -1: undecided
-    const int grid = (int)std::min<int64_t>(((int64_t)nc * 32 + 255) / 256, 148 * 16);
+    const int grid = (int)std::min<int64_t>(((int64_t)nc * 32 + 255) / 256, 132 * 16);
     const int BATCH = 4;  // rounds per host round trip
     int left[BATCH];
     for (int64_t round = 0; round < (int64_t)nc + BATCH; round += BATCH) {

@@ -335,7 +335,7 @@ __global__ void k_any_nonzero(const uint8_t *__restrict__ f, int64_t n, int *__r
 static int grid_for(int64_t work, int block) {
   int64_t g = (work + block - 1) / block;
   if (g < 1) g = 1;
-  if (g > 148 * 32) g = 148 * 32;
+  if (g > 132 * 32) g = 132 * 32;
   return (int)g;
 }
 

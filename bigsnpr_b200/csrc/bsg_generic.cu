@@ -148,7 +148,7 @@ __global__ void k_multlinreg(const uint8_t *__restrict__ raw, int64_t n_tot, con
   }
 }
 
-static int grid_warps(long long items) { return (int)std::max<long long>(1, std::min<long long>((items * 32 + 255) / 256, 148 * 16)); }
+static int grid_warps(long long items) { return (int)std::max<long long>(1, std::min<long long>((items * 32 + 255) / 256, 132 * 16)); }
 
 }  // namespace gen
 

@@ -1,4 +1,4 @@
-// bsg_gram5.cu -- the integer Gram tile on the 5th-generation tensor cores (tcgen05 + TMEM).
+// bsg_gram5.cu -- the integer Gram tile on the Hopper tensor cores (wgmma, register accumulators).
 //
 //   S[i][j] = sum_k code(i, k) * code(j, k)      for a 128 x 128 tile of lines, exact int32
 //
@@ -9,12 +9,12 @@
 //   8 producer warps : stream the packed lines (2 x LDG.128 = 128 codes per line and stage, register prefetch),
 //                      expand 2-bit codes to bytes with the class masks (w >> 2c) & 0x03030303 -- any fixed
 //                      permutation of k inside a 16-byte row is fine for a Gram product because both operands
-//                      use the same one -- and STS.128 them into shared memory in the UMMA canonical K-major
+//                      use the same one -- and STS.128 them into shared memory in the wgmma K-major
 //                      no-swizzle layout: core matrix = 8 rows x 16 B, SBO = 128 B between 8-row groups,
 //                      LBO = 2048 B between core matrices along K; fence.proxy.async + mbarrier arrive.
-//   1 MMA thread     : waits for the stage, issues 4 x tcgen05.mma.cta_group::1.kind::i8 (M = 128, N = 128,
-//                      K = 32, u8 x u8 -> s32 accumulator in TMEM), tcgen05.commit -> frees the stage.
-//   4 epilogue warps : tcgen05.ld 32x32b.x32 of the 128 x 128 int32 accumulator, 16-byte stores of the tile sums.
+//   2 consumer warpgroups: wait for the stage, each issues 4 x wgmma.m64n128k32.s32.u8.u8 on its 64 rows of the
+//                      tile (int32 accumulators in registers), and hands the stage back once those MMAs completed;
+//                      the tile sums are stored from the registers.
 #include <stdint.h>
 #include <string.h>
 
@@ -25,19 +25,20 @@ namespace bsg {
 namespace gram5 {
 
 constexpr int T5M = 128, T5N = 128;      // tile of line pairs
-constexpr int KSTAGE = 128;              // codes per line per stage (32 packed bytes) = 4 MMAs of K = 32; 96 KB of
-                                         // stages -> 2 CTAs per SM (measured: 256-code stages halve occupancy, GRM 212 vs 135 ms)
+constexpr int KSTAGE = 128;              // codes per line per stage (32 packed bytes) = 4 MMAs of K = 32
 constexpr int SBYTES = KSTAGE / 4;       // packed bytes per line per stage
 constexpr int NW = KSTAGE / 16;          // packed words (= core matrices along K) per line per stage
 constexpr int STAGES = 3;
 constexpr int PF = 2;                    // stages of register prefetch per producer thread
 constexpr int PROD_WARPS = 8;            // 256 producer threads: thread t expands line t (0..127 A, 128..255 B)
-constexpr int THREADS = (PROD_WARPS + 1) * 32;
+constexpr int MMA_WARPS = 8;             // two consumer warpgroups, 64 tile rows each
+// registers per thread after the split (65,536 in all): the consumers hold 64 int32 accumulators each
+constexpr int PROD_REGS = 96, MMA_REGS = 160;
+constexpr int THREADS = (PROD_WARPS + MMA_WARPS) * 32;
 constexpr int OPER_BYTES = 128 * KSTAGE;  // 16 KB per operand and stage
 constexpr int STAGE_BYTES = 2 * OPER_BYTES;
 constexpr int LBO = 2048, SBO = 128;     // bytes: next core matrix along K / along M
 constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 256;
-constexpr int TMEM_COLS = 128;
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
@@ -61,62 +62,55 @@ __device__ __forceinline__ void sts128(uint32_t addr, uint32_t a, uint32_t b, ui
   asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
 }
 
-// shared-memory matrix descriptor, K-major, SWIZZLE_NONE (cute::UMMA::SmemDescriptor): start >> 4 at [0,14),
-// LBO >> 4 at [16,30), SBO >> 4 at [32,46), version = 1 at [46,48), layout type 0 at [61,64)
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
-  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(LBO >> 4) << 16) | ((uint64_t)(SBO >> 4) << 32) | (1ull << 46);
-}
-
-// instruction descriptor (cute::UMMA::InstrDescriptor): c_format S32 = 2 at [4,6), a/b format U8 = 0, K-major both,
-// n_dim = N >> 3 at [17,23), m_dim = M >> 4 at [24,29)
-constexpr uint32_t IDESC = (2u << 4) | ((uint32_t)(T5N >> 3) << 17) | ((uint32_t)(T5M >> 4) << 24);
-
-__device__ __forceinline__ void umma_i8(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(da), "l"(db), "r"(IDESC), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-
 using Tile5 = gram::Tile;  // {i0, j0, mode, out}: out = offset (int32) of the 128 x 128 sums of this tile
+
+// consumer side of one pass over the contraction: warpgroup cw (0, 1) multiplies rows [64 cw, 64 cw + 64) of the A
+// stage by the 128 B rows; each stage is handed back to the producers once the MMAs reading it have completed
+__device__ __forceinline__ void consume_pass(uint32_t (&d)[64], uint32_t sbase, uint32_t bar, int nsteps, int cw, int lane,
+                                             int &stage, uint32_t &phase) {
+  int prev = -1;
+  for (int st = 0; st < nsteps; st++) {
+    mbar_wait(bar + 8 * stage, phase);
+    wg::fence();
+    const uint32_t a0 = sbase + stage * STAGE_BYTES + cw * 8 * SBO, b0 = sbase + stage * STAGE_BYTES + OPER_BYTES;
+#pragma unroll
+    for (int kk = 0; kk < KSTAGE / 32; kk++)
+      wg::mma_u8_n128(d, wg::desc(a0 + kk * 2 * LBO, LBO, SBO, 0), wg::desc(b0 + kk * 2 * LBO, LBO, SBO, 0), (st | kk) ? 1u : 0u);
+    wg::commit();
+    wg::wait<1>();  // the stage before this one has been read
+    if (prev >= 0 && lane == 0) mbar_arrive(bar + 8 * (STAGES + prev));
+    prev = stage;
+    if (++stage == STAGES) {
+      stage = 0;
+      phase ^= 1;
+    }
+  }
+  wg::wait<0>();
+  if (prev >= 0 && lane == 0) mbar_arrive(bar + 8 * (STAGES + prev));
+}
 
 __global__ void __launch_bounds__(THREADS, 1) k_gram5(const uint8_t *__restrict__ P, int64_t stride, int nlines,
                                                      int nsteps, const Tile5 *__restrict__ tiles,
                                                      int *__restrict__ sums) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  __shared__ uint32_t tmem_base_sh;
   const Tile5 t = tiles[blockIdx.x];
   if (t.mode != 0) return;  // tiles with missing values are done by the six-plane kernel
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t sbase = smem_u32(smem);
-  const uint32_t bar = sbase + STAGES * STAGE_BYTES;  // full[s] +8s, empty[s] +8(STAGES+s), done +8(2*STAGES)
+  const uint32_t bar = sbase + STAGES * STAGE_BYTES;  // full[s] +8s, empty[s] +8(STAGES+s)
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; s++) {
-      mbar_init(bar + 8 * s, PROD_WARPS);  // one arrive per producer warp
-      mbar_init(bar + 8 * (STAGES + s), 1);
+      mbar_init(bar + 8 * s, PROD_WARPS);            // one arrive per producer warp
+      mbar_init(bar + 8 * (STAGES + s), MMA_WARPS);  // one arrive per consumer warp
     }
-    mbar_init(bar + 8 * (2 * STAGES), 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == PROD_WARPS) {  // the MMA warp owns the TMEM allocation
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_sh)),
-                 "n"(TMEM_COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_d = tmem_base_sh;
 
   if (warp < PROD_WARPS) {
-    // ================= producers: packed line -> bytes in UMMA core-matrix layout =================
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(PROD_REGS));
+    // ================= producers: packed line -> bytes in the K-major core-matrix layout =================
     const int row = threadIdx.x & 127;         // row of the operand tile
     const int oper = threadIdx.x >> 7;         // 0: A lines (i0 + row), 1: B lines (j0 + row)
     int line = (oper ? t.j0 : t.i0) + row;
@@ -165,75 +159,37 @@ __global__ void __launch_bounds__(THREADS, 1) k_gram5(const uint8_t *__restrict_
         }
       }
     }
-  } else if (lane == 0) {
-    // ================= MMA issuer =================
+  } else {
+    // ================= two consumer warpgroups: MMAs, then the int32 sums straight from the registers =================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(MMA_REGS));
+    const int cw = (warp - PROD_WARPS) >> 2, wq = warp & 3;
+    uint32_t d[64];
     int stage = 0;
     uint32_t phase = 0;
-    for (int st = 0; st < nsteps; st++) {
-      mbar_wait(bar + 8 * stage, phase);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t a0 = sbase + stage * STAGE_BYTES, b0 = a0 + OPER_BYTES;
+    consume_pass(d, sbase, bar, nsteps, cw, lane, stage, phase);
+    int *out = sums + t.out;
 #pragma unroll
-      for (int kk = 0; kk < KSTAGE / 32; kk++) {
-        umma_i8(tmem_d, make_desc(a0 + kk * 2 * LBO), make_desc(b0 + kk * 2 * LBO), (st | kk) ? 1u : 0u);
-      }
-      umma_commit(bar + 8 * (STAGES + stage));  // stage reusable once these MMAs have read it
-      if (++stage == STAGES) {
-        stage = 0;
-        phase ^= 1;
-      }
+    for (int j = 0; j < 64; j += 2) {
+      const int r = 64 * cw + wg::acc_row(wq, lane, j), c = wg::acc_col(lane, j);
+      *reinterpret_cast<int2 *>(out + (int64_t)r * T5N + c) = make_int2((int)d[j], (int)d[j + 1]);
     }
-    umma_commit(bar + 8 * (2 * STAGES));  // accumulator complete
-  }
-
-  // ================= epilogue: TMEM -> registers -> global (warps 0..3 own TMEM lanes 32w..32w+31) =================
-  if (warp < 4) {
-    mbar_wait(bar + 8 * (2 * STAGES), 0);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const int r = warp * 32 + lane;
-    int *out = sums + t.out + (int64_t)r * T5N;
-#pragma unroll
-    for (int c0 = 0; c0 < T5N; c0 += 32) {
-      uint32_t v[32];
-      const uint32_t taddr = tmem_d + ((uint32_t)(warp * 32) << 16) + c0;
-      asm volatile(
-          "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-          "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-          : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-            "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-            "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-            "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-          : "r"(taddr));
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-      for (int q = 0; q < 8; q++)
-        *reinterpret_cast<uint4 *>(out + c0 + 4 * q) = make_uint4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-    }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == PROD_WARPS) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_d), "n"(TMEM_COLS) : "memory");
   }
 }
 
 }  // namespace gram5
 
 // ===================================================================================================
-// Weighted Gram on tcgen05 for bed_tcrossprodSelf:  K[i][j] += scale * sum_k fA(code(i,k)) * fB(code(j,k)) * d_k
+// Weighted Gram on wgmma for bed_tcrossprodSelf:  K[i][j] += scale * sum_k fA(code(i,k)) * fB(code(j,k)) * d_k
 // One CTA per 128 x 128 tile of the lower triangle; passes = weight slices x plane products, each pass a
-// full sweep over k with its own TMEM accumulator (two accumulators, ping-pong), so the epilogue of pass p
-// (TMEM -> registers -> K += scale * S) overlaps the MMAs of pass p + 1.
-//   warps 0..7  producers (as k_gram5; the B operand bytes are code * digit: ((x & 1) ? d : 0) | ((x & 2) ? 2d : 0))
-//   warp  8     MMA issuer + TMEM owner
-//   warps 9..12 epilogue (TMEM lane quarter = warp % 4)
+// full sweep over k into the consumers' register accumulators, then K += scale * S from those registers.  The
+// producers run ahead into the next pass's stages while the consumers fold the previous one into K.
+//   warps 0..7   producers (as k_gram5; the B operand bytes are code * digit: ((x & 1) ? d : 0) | ((x & 2) ? 2d : 0))
+//   warps 8..15  two consumer warpgroups (wgmma + epilogue, 64 tile rows each)
 // ===================================================================================================
 namespace wg5 {
 using namespace gram5;
 
-constexpr int EPI_WARPS = 4;
-constexpr int W5_THREADS = (PROD_WARPS + 1 + EPI_WARPS) * 32;
-constexpr int W5_TMEM_COLS = 256;  // 2 accumulators of 128 columns
+constexpr int W5_THREADS = THREADS;
 constexpr int W5_SMEM_BYTES = STAGES * STAGE_BYTES + 256;
 
 struct W5Tile {
@@ -277,7 +233,6 @@ __device__ __forceinline__ uint32_t cor_plane(uint32_t x, int pl) {
 template <int KIND>
 __global__ void __launch_bounds__(W5_THREADS, 1) k_wgram5(const W5Args a) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  __shared__ uint32_t tmem_base_sh;
   W5Tile t;
   long long out_off = 0;
   if (KIND == 0) {
@@ -290,34 +245,20 @@ __global__ void __launch_bounds__(W5_THREADS, 1) k_wgram5(const W5Args a) {
   }
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t sbase = smem_u32(smem);
-  const uint32_t bar = sbase + STAGES * STAGE_BYTES;
-  // full[s] +8s | empty[s] +8(STAGES+s) | acc_full[b] +8(2*STAGES+b) | acc_empty[b] +8(2*STAGES+2+b)
-  const uint32_t bar_accfull = bar + 8 * (2 * STAGES), bar_accempty = bar + 8 * (2 * STAGES + 2);
+  const uint32_t bar = sbase + STAGES * STAGE_BYTES;  // full[s] +8s | empty[s] +8(STAGES+s)
   const int npass = KIND == 1 ? 6 : (t.mode == 0 ? a.nslices : 4 * a.nslices);
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; s++) {
-      mbar_init(bar + 8 * s, PROD_WARPS);  // one arrive per producer warp
-      mbar_init(bar + 8 * (STAGES + s), 1);
-    }
-    for (int b = 0; b < 2; b++) {
-      mbar_init(bar_accfull + 8 * b, 1);
-      mbar_init(bar_accempty + 8 * b, EPI_WARPS * 32);
+      mbar_init(bar + 8 * s, PROD_WARPS);            // one arrive per producer warp
+      mbar_init(bar + 8 * (STAGES + s), MMA_WARPS);  // one arrive per consumer warp
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == PROD_WARPS) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_sh)),
-                 "n"(W5_TMEM_COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_d = tmem_base_sh;
 
   if (warp < PROD_WARPS) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(PROD_REGS));
     // ================= producers =================
     const int row = threadIdx.x & 127, oper = threadIdx.x >> 7;
     int line = (oper ? t.j0 : t.i0) + row;
@@ -395,79 +336,33 @@ __global__ void __launch_bounds__(W5_THREADS, 1) k_wgram5(const W5Args a) {
         }
       }
     }
-  } else if (warp == PROD_WARPS) {
-    // ================= MMA issuer =================
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int pass = 0; pass < npass; pass++) {
-        const int buf = pass & 1;
-        const uint32_t use = (uint32_t)(pass >> 1);           // n-th use of this accumulator
-        mbar_wait(bar_accempty + 8 * buf, (use & 1) ^ 1);     // epilogue of the previous use has drained it
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t acc = tmem_d + buf * 128;
-        for (int st = 0; st < a.nsteps; st++) {
-          mbar_wait(bar + 8 * stage, phase);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint32_t a0 = sbase + stage * STAGE_BYTES, b0 = a0 + OPER_BYTES;
-#pragma unroll
-          for (int kk = 0; kk < KSTAGE / 32; kk++)
-            umma_i8(acc, make_desc(a0 + kk * 2 * LBO), make_desc(b0 + kk * 2 * LBO), (st | kk) ? 1u : 0u);
-          umma_commit(bar + 8 * (STAGES + stage));
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        umma_commit(bar_accfull + 8 * buf);
-      }
-    }
   } else {
-    // ================= epilogue warps: K += scale * S =================
-    const int q4 = warp & 3;             // TMEM lane quarter of this warp
-    const int i = t.i0 + q4 * 32 + lane; // output row of this thread
+    // ================= consumer warpgroups: one pass of MMAs, then K += scale * S (or the int32 sums) =================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(MMA_REGS));
+    const int cw = (warp - PROD_WARPS) >> 2, wq = warp & 3;
+    int stage = 0;
+    uint32_t phase = 0;
+    uint32_t d[64];
     for (int pass = 0; pass < npass; pass++) {
       int prod = pass, slice = 0, wsel = 0;
       if (KIND == 0) pass_info(t.mode, a.nslices, pass, prod, slice, wsel);
-      const double sc = KIND == 0 ? a.scale[wsel][slice] : 0.0;
-      const int buf = pass & 1;
-      const uint32_t use = (uint32_t)(pass >> 1);
-      mbar_wait(bar_accfull + 8 * buf, use & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll 1
-      for (int c0 = 0; c0 < T5N; c0 += 32) {
-        uint32_t v[32];
-        const uint32_t taddr = tmem_d + ((uint32_t)(q4 * 32) << 16) + buf * 128 + c0;
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-            "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-            : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-              "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-              "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-              "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-            : "r"(taddr));
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        if (KIND == 0) {
+      consume_pass(d, sbase, bar, a.nsteps, cw, lane, stage, phase);
+      if (KIND == 0) {
+        const double sc = a.scale[wsel][slice];
 #pragma unroll
-          for (int e = 0; e < 32; e++) {
-            const int j = t.j0 + c0 + e;
-            if (i < a.nlines && j < a.nlines && i >= j) a.K[(int64_t)j * a.ldk + i] += sc * (double)(int)v[e];
-          }
-        } else {
-          int *dst = a.sums + out_off + (int64_t)pass * (T5M * T5N) + (int64_t)(q4 * 32 + lane) * T5N + c0;
+        for (int j = 0; j < 64; j++) {
+          const int i = t.i0 + 64 * cw + wg::acc_row(wq, lane, j), jj = t.j0 + wg::acc_col(lane, j);
+          if (i < a.nlines && jj < a.nlines && i >= jj) a.K[(int64_t)jj * a.ldk + i] += sc * (double)(int)d[j];
+        }
+      } else {
+        int *dst = a.sums + out_off + (int64_t)pass * (T5M * T5N);
 #pragma unroll
-          for (int e4 = 0; e4 < 8; e4++)
-            *reinterpret_cast<uint4 *>(dst + 4 * e4) = make_uint4(v[4 * e4], v[4 * e4 + 1], v[4 * e4 + 2], v[4 * e4 + 3]);
+        for (int j = 0; j < 64; j += 2) {
+          const int r = 64 * cw + wg::acc_row(wq, lane, j), c = wg::acc_col(lane, j);
+          *reinterpret_cast<int2 *>(dst + (int64_t)r * T5N + c) = make_int2((int)d[j], (int)d[j + 1]);
         }
       }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      mbar_arrive(bar_accempty + 8 * buf);
     }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == PROD_WARPS) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_d), "n"(W5_TMEM_COLS) : "memory");
   }
 }
 

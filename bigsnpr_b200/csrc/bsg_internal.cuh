@@ -154,11 +154,11 @@ int compact_lines(const uint8_t *src, int64_t src_stride, const int *code_idx, i
                   int nlines, uint8_t *out, int64_t out_stride, cudaStream_t s);
 int line_counts(const uint8_t *P, int64_t stride, int nlines, int L, int32_t *cnt, uint8_t *na, cudaStream_t s);
 
-// ---- bsg_gram5.cu: 128 x 128 integer Gram tiles on tcgen05 / TMEM (tiles = gram::Tile array on the device)
+// ---- bsg_gram5.cu: 128 x 128 integer Gram tiles on wgmma (tiles = gram::Tile array on the device)
 int gram5_launch(const uint8_t *P, int64_t stride, int nlines, int64_t line_bytes, const void *d_tiles, int ntiles,
                  int *d_sums, bool any_clean, bool any_na, cudaStream_t s);
 
-// weighted Gram for the GRM on tcgen05: tiles = (i0, j0, mode) int triplets on the host, K pre-zeroed, fills i >= j
+// weighted Gram for the GRM on wgmma: tiles = (i0, j0, mode) int triplets on the host, K pre-zeroed, fills i >= j
 int wgram5_launch(const uint8_t *P, int64_t stride, int nlines, int nslices, const uint8_t *const dig[3],
                   int64_t dig_stride, const double (*scale)[10], const int *h_tiles, int ntiles, double *K,
                   int64_t ldk, cudaStream_t s);
@@ -185,7 +185,7 @@ int generic_pairs(bsg_bed *h, const int *d_row, int nr, const int *d_col, int nc
 int generic_multlinreg(bsg_bed *h, const int *d_row, int nr, const int *d_col, int nc, const double *d_U, int K,
                        double *d_out, cudaStream_t s);
 
-// ---- bsg_gramt.cu: integer Gram tiles fed by TMA, 2-CTA tcgen05 MMAs (GRM and windowed correlations) ----------
+// ---- bsg_gramt.cu: integer Gram tiles fed by TMA, wgmma MMAs (GRM and windowed correlations) ----------
 namespace gram { struct Tile; }
 bool gramt_enabled();  // BSG_GRAM_TMA=0 selects the round-1 kernels (in-kernel expansion) for cross-checks
 int gramt_grm(const uint8_t *P, int64_t stride, int nr, int nc, const double *const Ws[3], const double wmax[3],

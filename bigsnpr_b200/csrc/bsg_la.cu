@@ -9,7 +9,7 @@
 //                   bsg_view_{c,}prodvec_dev.  Only ncv+1 doubles cross PCIe per step.
 //   bsg_tcrossprod  bed_tcrossprodSelf (R/bed-tcrossprodSelf.R:21-52): K = sum_blocks X~_b X~_b^T as ONE weighted
 //                   integer Gram product: the per-SNP weights 1/s^2, c/s^2, c^2/s^2 are quantised to base-64 digit
-//                   slices folded into the B bytes, the 128 x 128 tiles run on tcgen05 / TMEM (bsg_gram5.cu,
+//                   slices folded into the B bytes, the 128 x 128 tiles run on wgmma (bsg_gram5.cu,
 //                   k_wgram5) or on the register-IMMA kernel below (k_wgram), the centering terms come from two
 //                   matvecs.  The sample-major copy is built on demand.  Fallback (degenerate scaling, no room for
 //                   that copy): device decode of column blocks + cuBLAS DSYRK.
@@ -800,7 +800,7 @@ static int tcrossprod_dsyrk(bsg_bed *h, const int *ind_row, int nr, const int *i
       rc = fail(BSG_ERR_CUDA, "cublasDsyrk failed");
   }
   if (!rc && nr > 0) {
-    k_mirror_lower<<<(int)std::min<int64_t>(((int64_t)nr * nr + 255) / 256, 148 * 32), 256, 0, s>>>(dK, nr);
+    k_mirror_lower<<<(int)std::min<int64_t>(((int64_t)nr * nr + 255) / 256, 132 * 32), 256, 0, s>>>(dK, nr);
     count_launch();
     cudaError_t e2 = cudaGetLastError();
     if (K) prefault_pages(K, (size_t)nr * nr * sizeof(double));
@@ -916,7 +916,7 @@ static int tcrossprod_impl(bsg_bed *h, const int *ind_row, int nr, const int *in
   if (!K_dev) BSG_TRY(mem.alloc(&dK, (size_t)nr * nr));
   BSG_CUDA(cudaMemsetAsync(dK, 0, (size_t)nr * nr * sizeof(double), s));
   if (gramt_enabled() && nslices <= 4) {
-    // TMA-fed 2-CTA tcgen05 tiles over operands expanded once to uint8 (bsg_gramt.cu): all digit slices in one pass
+    // TMA-fed wgmma tiles over operands expanded once to uint8 (bsg_gramt.cu): all digit slices in one launch
     const double *Ws3[3] = {W1, W2p, W3};
     const double wmax[3] = {stats[0], stats[1], stats[2]};
     BSG_TRY(gramt_grm(P, stride, nr, nc, Ws3, wmax, na.data(), nslices, dK, nr, h->device, s));
@@ -936,7 +936,7 @@ static int tcrossprod_impl(bsg_bed *h, const int *ind_row, int nr, const int *in
     int ex = 0;
     if (stats[wv] > 0) frexp(stats[wv], &ex);
     const int e = dbits * nslices - 1 - ex;
-    k_weight_digits<<<(int)std::min<int64_t>(((int64_t)nchunks * 256 + 255) / 256, 148 * 16), 256, 0, s>>>(Ws[wv], nc, nchunks,
+    k_weight_digits<<<(int)std::min<int64_t>(((int64_t)nchunks * 256 + 255) / 256, 132 * 16), 256, 0, s>>>(Ws[wv], nc, nchunks,
                                                                                                         nslices, e, dbits, dg);
     count_launch();
     a.dig[wv] = dg;
@@ -954,7 +954,7 @@ static int tcrossprod_impl(bsg_bed *h, const int *ind_row, int nr, const int *in
   std::vector<uint8_t> na_jb(njb, 0);
   for (int i = 0; i < nr; i++) na_jb[i / TNv] |= na[i];
   if (use_t5) {
-    // 128 x 128 tiles on tcgen05 / TMEM (bsg_gram5.cu); digits are laid out 16 bytes per packed word, in order
+    // 128 x 128 wgmma tiles (bsg_gram5.cu); digits are laid out 16 bytes per packed word, in order
     std::vector<int> trip;
     for (int i0 = 0; i0 < nr; i0 += 128) {
       const bool na_i = na_jb[i0 / 128] != 0;
@@ -1019,7 +1019,7 @@ static int tcrossprod_impl(bsg_bed *h, const int *ind_row, int nr, const int *in
     }
   }
   if (!rc) {
-    k_grm_finish<<<(int)std::min<int64_t>(((int64_t)nr * nr + 255) / 256, 148 * 32), 256, 0, s>>>(dK, nr, nr, d_r, d_q, sumW3);
+    k_grm_finish<<<(int)std::min<int64_t>(((int64_t)nr * nr + 255) / 256, 132 * 32), 256, 0, s>>>(dK, nr, nr, d_r, d_q, sumW3);
     count_launch();
     cudaError_t e2 = cudaGetLastError();
     if (K) prefault_pages(K, (size_t)nr * nr * sizeof(double));  // 800 MB at configs[3], while the device still computes

@@ -424,7 +424,7 @@ __global__ void k_apply(const long long *__restrict__ outN, const int *__restric
   part[(int64_t)l * 16 + 12] = outN[phys * 2 + 1];
 }
 
-static int grid_cap(int64_t work, int block) { return (int)std::max<int64_t>(1, std::min<int64_t>((work + block - 1) / block, 148 * 32)); }
+static int grid_cap(int64_t work, int block) { return (int)std::max<int64_t>(1, std::min<int64_t>((work + block - 1) / block, 132 * 32)); }
 
 }  // namespace naell
 
@@ -549,7 +549,7 @@ bool na_ell_ready(bsg_bed *h) {
 int na_ell_correction(bsg_bed *h, int side, const int *lines, int nlines, const long long *Q, long long *part, cudaStream_t s) {
   using namespace naell;
   if (nlines <= 0) return BSG_OK;
-  int nsm = 148;
+  int nsm = 132;
   cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, h->device);
   const int ngroups = h->ellGroups[side], nchunks = h->ellChunks[side];
   // two CTAs of 16 warps per SM: few groups -> one group per warp and the chunks split over several CTAs (one resident

@@ -197,7 +197,7 @@ __global__ void k_pack_bed(const uint8_t *__restrict__ A, int64_t strideA, const
   }
 }
 
-static int grid1(int64_t work, int block, int cap = 148 * 16) {
+static int grid1(int64_t work, int block, int cap = 132 * 16) {
   int64_t g = (work + block - 1) / block;
   if (g < 1) g = 1;
   if (g > cap) g = cap;
@@ -216,7 +216,7 @@ int simple_cprodvec(bsg_bed *h, const int *d_row, int nr, const int *d_col, int 
 static int simple_prodvec_any(bsg_bed *h, const int *d_row, int nr, const int *d_col, int nc, const double *d_center,
                               const double *d_scale, const double *d_x, double *d_out, cudaStream_t s, int square) {
   int gx = (nr + 255) / 256;
-  int nsplit = (148 * 8 + gx - 1) / gx;
+  int nsplit = (132 * 8 + gx - 1) / gx;
   int max_split = (nc + 127) / 128;
   if (nsplit > max_split) nsplit = max_split;
   if (nsplit < 1) nsplit = 1;

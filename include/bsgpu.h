@@ -1,8 +1,8 @@
 /*
- * bsgpu.h -- C ABI of libbsgpu, the B200 (sm_100a) engine for bigsnpr's packed-genotype hot path.
+ * bsgpu.h -- C ABI of libbsgpu, the H100 (sm_90a) engine for bigsnpr's packed-genotype hot path.
  *
  * This is the drop-in boundary: plain pointers and sizes, no R / torch types.  Every entry point
- * replaces one `.Call` target of privefl/bigsnpr 1.12.21 (file:line under /root/reference cited per
+ * replaces one `.Call` target of privefl/bigsnpr 1.12.21 (file:line of the bigsnpr sources cited per
  * function); the R-side shim that binds them under the original `_bigsnpr_*` names is r_shim/ and
  * is documented in INTEGRATION.md.
  *

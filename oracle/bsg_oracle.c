@@ -2,7 +2,7 @@
  * bsg_oracle.c -- CPU restatement of the bigsnpr hot path.
  *
  * TEST INFRASTRUCTURE ONLY.  This file is the parity oracle and the CPU baseline
- * ("cpu_baseline.kind = port") for the B200 engine.  Only tests/, __graft_entry__.smoke()
+ * ("cpu_baseline.kind = port") for the H100 engine.  Only tests/, __graft_entry__.smoke()
  * and bench.py's cpu_baseline / --impl reference legs may load it.  The product
  * (libbsgpu.so) never links, loads or calls anything in this directory.
  *

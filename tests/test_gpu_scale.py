@@ -163,6 +163,57 @@ def test_cfg4_slice_grm_vs_oracle(B, oracle):
         g.close()
 
 
+_IN_KERNEL_EXPANSION_RUN = """
+import sys
+import numpy as np
+sys.path.insert(0, sys.argv[1])
+import bigsnpr_b200 as B
+
+out = {}
+pos = 1000.0 * np.arange(1, 1001)
+for na in (0.0, 0.005):
+    g = B.Bed.synthetic(20_000, 1_000, seed=31, na_rate=na, ld_rho=0.9, ld_block=50)
+    out["cor_%g" % na] = B.bed_cor(g, size=500, thr_r2=0.0, infos_pos=pos)
+    g.close()
+for na in (0.0, 0.01):
+    g = B.Bed.synthetic(3_000, 10_000, seed=41, na_rate=na)
+    out["grm_%g" % na] = B.bed_tcrossprodSelf(g)[0]
+    g.close()
+np.savez(sys.argv[2], **{k + "_%d" % j: v for k, vs in out.items() for j, v in enumerate(vs if isinstance(vs, tuple) else (vs,))})
+"""
+
+
+def test_in_kernel_expansion_gram_tiles_vs_oracle(B, oracle, tmp_path):
+    """The Gram kernels that expand the 2-bit codes inside the tile (bsg_gram5.cu: k_gram5, k_wgram5) serve bed_cor when
+    the expanded operand planes do not fit in HBM and the GRM with more than four weight digits.  BSG_GRAM_TMA=0 selects
+    them for the whole process (the switch is read once), hence the subprocess: windowed correlations with and without
+    missing values (missing-free tiles and six-plane tiles) and the weighted GRM, against the oracle."""
+    import os
+    import subprocess
+    import sys
+
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    res = tmp_path / "gram5.npz"
+    r = subprocess.run([sys.executable, "-c", _IN_KERNEL_EXPANSION_RUN, root, str(res)], capture_output=True, text=True,
+                       env=dict(os.environ, BSG_GRAM_TMA="0"), timeout=900)
+    assert r.returncode == 0, r.stderr[-3000:]
+    got = np.load(res)
+    nt = oracle.max_threads()
+    pos = 1000.0 * np.arange(1, 1001)
+    for na in (0.0, 0.005):
+        o = oracle.synth_bed(20_000, 1_000, seed=31, na_rate=na, ld_rho=0.9, ld_block=50)
+        p0, i0, x0 = oracle.cor0(o, size=500, thr_r2=0.0, infos_pos=pos, ncores=nt)
+        key = "cor_%g" % na
+        assert np.array_equal(got[key + "_0"], p0) and np.array_equal(got[key + "_1"], i0)
+        assert np.allclose(got[key + "_2"], x0, rtol=0, atol=1e-12)
+    for na in (0.0, 0.01):
+        o = oracle.synth_bed(3_000, 10_000, seed=41, na_rate=na)
+        K0 = oracle.bed_tcrossprodSelf(o, block_size=2000)[0]
+        K = got["grm_%g_0" % na]
+        assert np.max(np.abs(K - K0)) / np.max(np.abs(K0)) < 1e-8
+        assert np.array_equal(K, K.T)
+
+
 def test_products_on_the_default_stream_are_ordered(B):
     """ADVICE r1 (high): a NULL stream means the legacy default stream.  The product is enqueued between two torch
     operations on torch's default stream with no synchronisation in between; repeated with fresh inputs it must always see

@@ -1,8 +1,8 @@
-// ubench.cu -- microbenchmarks that size the design choices of k_pmv on a real B200:
-//   (1) IMMA.16832.U8.S8 issue rate per SM (legacy mma.sync path on sm_100a)
+// ubench.cu -- microbenchmarks that size the design choices of k_pmv on a real GPU:
+//   (1) IMMA.16832.U8.S8 issue rate per SM (legacy mma.sync path on sm_90a)
 //   (2) cp.async.bulk (UBLKCP) throughput per SM as a function of the copy size
 //   (3) plain LDG.128 streaming bandwidth (for reference)
-// build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/ubench tools/ubench.cu
+// build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/ubench tools/ubench.cu
 #include <cstdint>
 #include <cstdio>
 #include <cuda_runtime.h>
@@ -72,14 +72,14 @@ __global__ void k_ldg(const uint4 *src, size_t n, uint4 *out) {
 }
 
 int main() {
-  int nsm = 148;
+  int nsm = 132;
   cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, 0);
   int clk = 0;
   cudaDeviceGetAttribute(&clk, cudaDevAttrClockRate, 0);
   printf("SMs %d, clock attr %d kHz\n", nsm, clk);
   int *out; long long *cyc;
-  CK(cudaMalloc(&out, 148 * 1024 * 4)); CK(cudaMalloc(&cyc, 148 * 8));
-  long long hc[148];
+  CK(cudaMalloc(&out, nsm * 1024 * 4)); CK(cudaMalloc(&cyc, nsm * 8));
+  long long hc[1024];
   cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
   // (1) IMMA
   for (int warps : {1, 4, 8, 16}) {
