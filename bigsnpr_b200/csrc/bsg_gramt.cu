@@ -299,6 +299,20 @@ __global__ void k_weight_digits_plain(const double *__restrict__ W, int64_t len,
 }
 
 // ---- host side ---------------------------------------------------------------------------------------------------------
+template <int EPI>
+static int launch(const CUtensorMap &mA, const CUtensorMap &mB, const GtArgs &a, int ntiles, cudaStream_t s) {
+  BSG_CUDA(cudaFuncSetAttribute(k_gramt<EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
+  k_gramt<EPI><<<2 * ntiles, THREADS, SMEM, s>>>(mA, mB, a);
+  count_launch();
+  BSG_CUDA(cudaGetLastError());
+  return BSG_OK;
+}
+
+static int grid_cap(int64_t work) { return (int)std::max<int64_t>(1, std::min<int64_t>((work + 255) / 256, 132 * 32)); }
+
+}  // namespace gt
+
+// ---- tensor maps ---------------------------------------------------------------------------------------------------
 typedef CUresult (*EncodeFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
                              const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle,
                              CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -312,30 +326,18 @@ static EncodeFn encode_fn() {
   }
   return fn;
 }
-// rows x pitch bytes, row-major, box = 128 bytes x 128 rows, 128-byte swizzle, rows beyond `rows` read as zero
-static int make_map(CUtensorMap *m, const uint8_t *base, int64_t rows, int64_t pitch) {
+// rows x pitch bytes, row-major, box = 128 bytes x box_rows rows, 128-byte swizzle, L2 promotion to 256 B; boxes
+// reaching past `rows` or `pitch` read as zero.  Shared by the Gram tiles and k_pmvT (bsg_pmv.cu).
+int make_map(CUtensorMap *m, const uint8_t *base, int64_t rows, int64_t pitch, int box_rows) {
   EncodeFn f = encode_fn();
   if (!f) return fail(BSG_ERR_CUDA, "cuTensorMapEncodeTiled is not available from this driver.");
   cuuint64_t gdim[2] = {(cuuint64_t)pitch, (cuuint64_t)rows}, gstr[1] = {(cuuint64_t)pitch};
-  cuuint32_t box[2] = {(cuuint32_t)BK, (cuuint32_t)BM}, estr[2] = {1, 1};
+  cuuint32_t box[2] = {128, (cuuint32_t)box_rows}, estr[2] = {1, 1};
   CUresult r = f(m, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, (void *)base, gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                  CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return fail(BSG_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d).", (int)r);
   return BSG_OK;
 }
-
-template <int EPI>
-static int launch(const CUtensorMap &mA, const CUtensorMap &mB, const GtArgs &a, int ntiles, cudaStream_t s) {
-  BSG_CUDA(cudaFuncSetAttribute(k_gramt<EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
-  k_gramt<EPI><<<2 * ntiles, THREADS, SMEM, s>>>(mA, mB, a);
-  count_launch();
-  BSG_CUDA(cudaGetLastError());
-  return BSG_OK;
-}
-
-static int grid_cap(int64_t work) { return (int)std::max<int64_t>(1, std::min<int64_t>((work + 255) / 256, 132 * 32)); }
-
-}  // namespace gt
 
 bool gramt_enabled() {
   static int on = -1;
@@ -422,9 +424,9 @@ int gramt_grm(const uint8_t *P, int64_t stride, int nr, int nc, const double *co
     const int64_t klen = std::min<int64_t>(kblk, nc - k0);
     const int64_t pitch = round_up(klen, BK);
     CUtensorMap mAa, mAn, mB;
-    BSG_TRY(make_map(&mAa, Aa, lines_pad, pitch));
-    if (any_na) BSG_TRY(make_map(&mAn, An, lines_pad, pitch));
-    BSG_TRY(make_map(&mB, Bw, (int64_t)nslices * lines_pad, pitch));
+    BSG_TRY(make_map(&mAa, Aa, lines_pad, pitch, BM));
+    if (any_na) BSG_TRY(make_map(&mAn, An, lines_pad, pitch, BM));
+    BSG_TRY(make_map(&mB, Bw, (int64_t)nslices * lines_pad, pitch, BM));
     k_expand_plane<<<grid_cap((int64_t)nr * (pitch / 16)), 256, 0, s>>>(P, stride, nr, k0, pitch, any_na ? 0 : 4, Aa, 0);
     if (any_na) k_expand_plane<<<grid_cap((int64_t)nr * (pitch / 16)), 256, 0, s>>>(P, stride, nr, k0, pitch, 1, An, 0);
     count_launch(any_na ? 2 : 1);
@@ -500,7 +502,7 @@ int gramt_cor(const uint8_t *M, int64_t stride, int nlines, const gram::Tile *ti
     count_launch();
   }
   CUtensorMap mE;  // A and B tiles are both rows of the expanded planes
-  BSG_TRY(make_map(&mE, E, (int64_t)nplanes * lines_pad, pitch));
+  BSG_TRY(make_map(&mE, E, (int64_t)nplanes * lines_pad, pitch, BM));
   // group the 128 x 128 tiles: pairs of row blocks (256 rows) x runs of up to four column blocks.  The list is ordered by
   // row block, then column block (bsg_cor.cu), so a row block's tiles are consecutive.
   struct Key { int i0, j0, idx; };

@@ -11,6 +11,7 @@
 //   * copy B (sample-major), optional: line i = sample i, m codes.  Line stride = round_up(ceil(m/4), 128).
 //     Built on request or on first use by the GRM; every other kernel runs from copy A alone.
 #pragma once
+#include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <string>
@@ -192,6 +193,8 @@ int gramt_grm(const uint8_t *P, int64_t stride, int nr, int nc, const double *co
               const uint8_t *na, int nslices, double *K, int64_t ldk, int device, cudaStream_t s);
 int gramt_cor(const uint8_t *M, int64_t stride, int nlines, const gram::Tile *tiles, int ntiles, int *d_sums, int device,
               cudaStream_t s, bool *done);
+// TMA map over rows x pitch bytes: 128 B x box_rows boxes, 128-byte swizzle, zero fill out of bounds
+int make_map(CUtensorMap *m, const uint8_t *base, int64_t rows, int64_t pitch, int box_rows);
 
 // ---- bsg_pmv.cu: packed matrix x vector on the integer tensor pipe ----------------------------
 struct PmvPlan;  // opaque, owned by a view

@@ -805,11 +805,11 @@ static int run_pmv(bsg_view *v, const uint8_t *P, int64_t stride, int L, const i
 //
 // The contraction now runs ACROSS lines (SNPs) while the bytes of a line run along samples, so the IMMA k index
 // has to be assembled from 4 different lines.  A CTA owns TBYTES sample-bytes (4 TBYTES samples) of every line,
-// 64 bytes per warp, and walks a range of lines 32 at a time: every warp stages its own 32 x 64 B strip with
-// cp.async into a private multi-stage ring (no block barrier in the loop), laid out so the fragment reads are
-// conflict free; every thread reads one 32-bit word from 4 consecutive lines and transposes the 4 x 4 bytes with
-// 8 PRMTs.  A transposed word holds, for 4 lines, the
-// byte of 4 samples: masking the 2-bit fields gives the A fragments of 4 IMMAs (sample 4b + c, c = 0..3; field c
+// 64 bytes per warp, and walks a range of lines 32 at a time.  k_pmvT (all lines in order) fills CTA-wide stages of
+// 32 lines x 512 B with 2D TMA boxes; k_pmvT_lines (a line list: TMA has no row gather on sm_90a) stages each warp's
+// own 32 x 64 B strip with cp.async.  Either way the fragment reads are conflict free; every thread reads one 32-bit
+// word from 4 consecutive lines and transposes the 4 x 4 bytes with 8 PRMTs.  A transposed word holds, for 4 lines,
+// the byte of 4 samples: masking the 2-bit fields gives the A fragments of 4 IMMAs (sample 4b + c, c = 0..3; field c
 // enters as 4^c x code, removed by an exact shift in the epilogue).  B = the 8 signed base-256 digits
 // of the quantised vector, 32 lines per step, laid out [step][slice][32] so a B register is one aligned word.
 // Per warp and step: 16 IMMAs over 32 lines x 64 bytes; accumulators: 4 (byte) x 4 (field) x 4 registers.
@@ -846,8 +846,9 @@ __device__ __forceinline__ uint32_t prmt(uint32_t a, uint32_t b, uint32_t sel) {
   return r;
 }
 
-template <int PLANE, bool LINES>
-__global__ void __launch_bounds__(TWARPS * 32, 2) k_pmvT(const TArgs a) {
+// Line list (a.lines): per-warp cp.async strips.
+template <int PLANE>
+__global__ void __launch_bounds__(TWARPS * 32, 2) k_pmvT_lines(const TArgs a) {
   extern __shared__ __align__(128) uint8_t smem[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, q = lane & 3;
   const int blk = blockIdx.x % a.nblocks, ks = blockIdx.x / a.nblocks;
@@ -871,15 +872,12 @@ __global__ void __launch_bounds__(TWARPS * 32, 2) k_pmvT(const TArgs a) {
     const int hf = row >> 4, qq = (row >> 2) & 3, r = row & 3, sl = lch >> 1, hc = lch & 1;
     dst_off[i] = (uint32_t)((((((r * 2 + hf) * 2 + sl) * 4 + qq) * 8) + 4 * hc) * 4);
   }
-  const int full_steps = (l1 - l0) / TLINES;  // steps whose 32 lines all exist
-  const int64_t stride8 = 8 * a.stride;
-  // general issue: any step, clamped rows, optional line list
   auto issue = [&](int step, int stage) {
     const uint32_t dst = wbase + stage * WSTAGE_BYTES;
 #pragma unroll
     for (int i = 0; i < 4; i++) {
       const int t = min(l0 + step * TLINES + 8 * i + lrow, l1 - 1);
-      const int phys = LINES ? a.lines[t] : t;
+      const int phys = a.lines[t];
       cp_async16(dst + dst_off[i], a.P + colb + (int64_t)phys * a.stride, 16);
     }
   };
@@ -943,35 +941,9 @@ __global__ void __launch_bounds__(TWARPS * 32, 2) k_pmvT(const TArgs a) {
     }
   };
 
-  int step = 0;
   uint32_t rd_stage = 0, wr_stage = (TSTAGES - 1) * WSTAGE_BYTES;  // byte offsets of the stage read / refilled
   const uint8_t *dgn = dg + 256;
-  // main loop (identity line order): the refilled step is entirely in range -> running pointers, no branches
-  if (!LINES) {
-    const int main_end = min(nsteps, full_steps - (TSTAGES - 1));
-    const uint8_t *psrc = a.P + colb + (int64_t)(l0 + (TSTAGES - 1) * TLINES + lrow) * a.stride;
-    for (; step < main_end; step++) {
-      asm volatile("cp.async.wait_group %0;" ::"n"(TSTAGES - 2) : "memory");
-      __syncwarp();
-      {
-        const uint32_t dst = wbase + wr_stage;
-        cp_async16(dst + dst_off[0], psrc, 16);
-        cp_async16(dst + dst_off[1], psrc + stride8, 16);
-        cp_async16(dst + dst_off[2], psrc + 2 * stride8, 16);
-        cp_async16(dst + dst_off[3], psrc + 3 * stride8, 16);
-        asm volatile("cp.async.commit_group;" ::: "memory");
-        psrc += 4 * stride8;
-      }
-      const uint32_t b0 = nb0, b1 = nb1;
-      nb0 = *reinterpret_cast<const uint32_t *>(dgn);  // main_end < nsteps: the next step exists
-      nb1 = *reinterpret_cast<const uint32_t *>(dgn + 16);
-      dgn += 256;
-      compute(rd_base + rd_stage, b0, b1);
-      rd_stage = rd_stage + WSTAGE_BYTES == TSTAGES * WSTAGE_BYTES ? 0 : rd_stage + WSTAGE_BYTES;
-      wr_stage = wr_stage + WSTAGE_BYTES == TSTAGES * WSTAGE_BYTES ? 0 : wr_stage + WSTAGE_BYTES;
-    }
-  }
-  for (; step < nsteps; step++) {
+  for (int step = 0; step < nsteps; step++) {
     asm volatile("cp.async.wait_group %0;" ::"n"(TSTAGES - 2) : "memory");
     __syncwarp();
     {
@@ -991,6 +963,156 @@ __global__ void __launch_bounds__(TWARPS * 32, 2) k_pmvT(const TArgs a) {
   }
   asm volatile("cp.async.wait_group 0;" ::: "memory");
   // epilogue: D rows = samples (slot g / g + 8), D columns = slices 2q, 2q + 1
+#pragma unroll
+  for (int j = 0; j < 4; j++)
+#pragma unroll
+    for (int c = 0; c < 4; c++)
+#pragma unroll
+      for (int sl = 0; sl < 2; sl++) {
+        const int64_t sample = 4 * (byte0 + 4 * (8 * sl + g) + j) + c;
+        if (sample < a.n) {
+          unsigned long long *dst = reinterpret_cast<unsigned long long *>(a.part) + sample * 16 + (PLANE ? 8 : 0) + 2 * q;
+          long long v0 = acc[j][c][2 * sl], v1 = acc[j][c][2 * sl + 1];
+          v0 >>= 2 * c;
+          v1 >>= 2 * c;
+          if (v0) atomicAdd(dst, (unsigned long long)v0);
+          if (v1) atomicAdd(dst + 1, (unsigned long long)v1);
+        }
+      }
+}
+
+// All lines in order: CTA-wide stages.  A stage is the CTA's 512-byte segment of 32 consecutive lines as 4 TMA boxes
+// of 32 rows x 128 B (128-byte swizzle: 16-byte chunk c of row R sits at chunk c ^ (R & 7)), plus the step's 256-byte
+// digit block (slices 4..7 shifted by 16 B).  Thread 0 fills the stages, full / empty mbarriers track them, so the warps
+// run no per-lane loader code and read both operands from shared memory (a dedicated producer warp would make 9 warps
+// per CTA and cap the registers at 96: the accumulators alone take 64).  Rows past the selected lines and
+// columns past the line stride arrive as zeros (and rows past the last selected line meet zero digits anyway).
+// Consumer lane (g, q) of warp w reads word column 16 (w & 1) + 8 sl + g of box w >> 1 in rows 16 hf + 4 q + r; lanes
+// with q >= 2 read a quad's rows in the order 2, 3, 0, 1, so every 32-lane LDS hits 32 distinct banks, and the last
+// PRMTs of the transpose restore the order.
+constexpr int TBOX = 32 * 128;                               // one box: 32 rows x 128 B
+constexpr int TDIG_OFF = 4 * TBOX;
+constexpr int TSTAGE_BYTES = 4 * TBOX + 1024;                // + digits; stages stay 1 KB aligned (swizzle atom)
+constexpr int TCSTAGES = 6;                                  // 100 KB of stages per CTA, 2 CTAs per SM
+constexpr int TSMEM_TMA = TCSTAGES * TSTAGE_BYTES + 2 * TCSTAGES * 8 + 1024;  // + mbarriers + alignment slack
+
+__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap *map, uint32_t bar, int c0, int c1) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(dst),
+      "l"(map), "r"(bar), "r"(c0), "r"(c1)
+      : "memory");
+}
+
+// address bits of read i (row i, chunk ^ i) and of word column half sl (chunk ^ 2 sl), relative to the lane's i = sl = 0
+__host__ __device__ constexpr uint32_t TRD(int i, int sl) { return (uint32_t)((i << 7) ^ (i << 4) ^ (sl << 5)); }
+
+template <int PLANE>
+__global__ void __launch_bounds__(TWARPS * 32, 2) k_pmvT(const __grid_constant__ CUtensorMap map, const TArgs a) {
+  extern __shared__ __align__(128) uint8_t smem[];
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, q = lane & 3;
+  const int blk = blockIdx.x % a.nblocks, ks = blockIdx.x / a.nblocks;
+  const int l0 = ks * a.lines_per_split, l1 = min(a.nlines, l0 + a.lines_per_split);
+  const int nsteps = (l1 - l0 + TLINES - 1) / TLINES;
+  const uint32_t sbase = (smem_u32(smem) + 1023u) & ~1023u;
+  const uint32_t bar_base = sbase + TCSTAGES * TSTAGE_BYTES;  // full[s] at +8s, empty[s] at +8(TCSTAGES+s)
+  // producer = thread 0: 4 boxes + 2 digit copies per stage
+  auto fill = [&](int step, int st) {
+    const uint32_t full = bar_base + 8 * st, dst = sbase + st * TSTAGE_BYTES;
+    const uint8_t *dg = a.dig + (int64_t)(l0 / TLINES + step) * 256;
+    mbar_expect_tx(full, 4 * TBOX + 256);
+#pragma unroll
+    for (int j = 0; j < 4; j++) tma_load_2d(dst + j * TBOX, &map, full, blk * TBYTES + 128 * j, l0 + step * TLINES);
+    bulk_g2s(dst + TDIG_OFF, dg, 128, full);
+    bulk_g2s(dst + TDIG_OFF + 144, dg + 128, 128, full);
+  };
+  if (tid == 0) {
+    for (int st = 0; st < TCSTAGES; st++) {
+      mbar_init(bar_base + 8 * st, 1);
+      mbar_init(bar_base + 8 * (TCSTAGES + st), TWARPS);
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    for (int st = 0; st < min(TCSTAGES, nsteps); st++) fill(st, st);
+  }
+  __syncthreads();
+  int stage = 0, pstage = 0;  // stage of this step / of the previous one
+  uint32_t phase = 0, pphase = 0;
+
+  const int64_t byte0 = (int64_t)blk * TBYTES + 64 * warp;  // this warp's 64 sample-bytes of every line
+  // Read i (row r = i ^ rsw of the quad) of word column 8 sl + g sits at row 4 q + r, chunk
+  // (4 (w & 1) + 2 sl + (g >> 2)) ^ (4 (q & 1) + r), word g & 3 of the box.  Row (bits 7-8), chunk (bits 4-6) and word
+  // (bits 2-3) are disjoint address fields of a 1 KB aligned box, so the (i, sl) part is an XOR with a constant.
+  const int rsw = 2 * (q >> 1);
+  const uint32_t chunk0 = (4 * (warp & 1) + (g >> 2)) ^ (4 * (q & 1) + rsw);
+  const uint32_t rd_base = sbase + (warp >> 1) * TBOX + q * 512 + (rsw << 7) + chunk0 * 16 + 4 * (g & 3);
+  const uint32_t dg_base = sbase + TDIG_OFF + g * 32 + 16 * (g >> 2) + 4 * q;  // slice g, lines 4q..4q+3
+  const uint32_t sel_lo = rsw ? 0x1054u : 0x5410u, sel_hi = rsw ? 0x3276u : 0x7632u;
+
+  int acc[4][4][4];
+#pragma unroll
+  for (int j = 0; j < 4; j++)
+#pragma unroll
+    for (int c = 0; c < 4; c++)
+#pragma unroll
+      for (int k = 0; k < 4; k++) acc[j][c][k] = 0;
+
+  for (int step = 0; step < nsteps; step++) {
+    const uint32_t full = bar_base + 8 * stage, empty = bar_base + 8 * (TCSTAGES + stage);
+    const uint32_t so = stage * TSTAGE_BYTES;
+    const int cstage = stage;
+    const uint32_t cphase = phase;
+    mbar_wait(full, phase);
+    const uint32_t b0 = lds32(dg_base + so), b1 = lds32(dg_base + so + 16);
+    uint32_t W[2][2][4];  // [slot g / g+8][lines lo / hi][byte]
+#pragma unroll
+    for (int sl = 0; sl < 2; sl++)
+#pragma unroll
+      for (int hf = 0; hf < 2; hf++) {
+        const uint32_t ad = rd_base + so, hb = hf * (16 * 128);
+        const uint32_t x0 = lds32((ad ^ TRD(0, sl)) + hb), x1 = lds32((ad ^ TRD(1, sl)) + hb);
+        const uint32_t x2 = lds32((ad ^ TRD(2, sl)) + hb), x3 = lds32((ad ^ TRD(3, sl)) + hb);
+        const uint32_t t0 = prmt(x0, x1, 0x5140), t1 = prmt(x2, x3, 0x5140);
+        const uint32_t t2 = prmt(x0, x1, 0x7362), t3 = prmt(x2, x3, 0x7362);
+        W[sl][hf][0] = prmt(t0, t1, sel_lo);
+        W[sl][hf][1] = prmt(t0, t1, sel_hi);
+        W[sl][hf][2] = prmt(t2, t3, sel_lo);
+        W[sl][hf][3] = prmt(t2, t3, sel_hi);
+      }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(empty);
+    if (++stage == TCSTAGES) {
+      stage = 0;
+      phase ^= 1;
+    }
+#pragma unroll
+    for (int j = 0; j < 4; j++) {
+      uint32_t wa = W[0][0][j], wb = W[1][0][j], wc2 = W[0][1][j], wd = W[1][1][j];
+      if (PLANE == 1) {
+        wa = wa & (wa >> 1) & 0x55555555u;
+        wb = wb & (wb >> 1) & 0x55555555u;
+        wc2 = wc2 & (wc2 >> 1) & 0x55555555u;
+        wd = wd & (wd >> 1) & 0x55555555u;
+      } else if (PLANE == 2) {
+        wa = (wa >> 1) & 0x55555555u;
+        wb = (wb >> 1) & 0x55555555u;
+        wc2 = (wc2 >> 1) & 0x55555555u;
+        wd = (wd >> 1) & 0x55555555u;
+      }
+      mma_u8s8(acc[j][0], wa & 0x03030303u, wb & 0x03030303u, wc2 & 0x03030303u, wd & 0x03030303u, b0, b1);
+      mma_u8s8(acc[j][1], wa & 0x0C0C0C0Cu, wb & 0x0C0C0C0Cu, wc2 & 0x0C0C0C0Cu, wd & 0x0C0C0C0Cu, b0, b1);
+      mma_u8s8(acc[j][2], wa & 0x30303030u, wb & 0x30303030u, wc2 & 0x30303030u, wd & 0x30303030u, b0, b1);
+      mma_u8s8(acc[j][3], wa & 0xC0C0C0C0u, wb & 0xC0C0C0C0u, wc2 & 0xC0C0C0C0u, wd & 0xC0C0C0C0u, b0, b1);
+    }
+    // refill one step behind: the previous step's stage, once all warps have released it.  The one-step slack keeps
+    // thread 0 from waiting on the slowest warp of the current step; TCSTAGES - 1 stages stay in flight.
+    if (tid == 0 && step >= 1 && step - 1 + TCSTAGES < nsteps) {
+      mbar_wait(bar_base + 8 * (TCSTAGES + pstage), pphase);
+      fill(step - 1 + TCSTAGES, pstage);
+    }
+    __syncwarp();
+    pstage = cstage;
+    pphase = cphase;
+  }
+  // epilogue: as k_pmvT_lines
 #pragma unroll
   for (int j = 0; j < 4; j++)
 #pragma unroll
@@ -1598,8 +1720,8 @@ static int run_pmvT(bsg_view *v, const uint8_t *dig_raw, int plane, const uint8_
   a.ksplit = (nc + a.lines_per_split - 1) / a.lines_per_split;
   static unsigned attr_done = 0;  // one bit per device: function attributes are per device
   if (!(attr_done >> (h->device & 31) & 1u)) {
-    BSG_CUDA(cudaFuncSetAttribute(k_pmvT<0, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, TSMEM));
-    BSG_CUDA(cudaFuncSetAttribute(k_pmvT<0, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TSMEM));
+    BSG_CUDA(cudaFuncSetAttribute(k_pmvT<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, TSMEM_TMA));
+    BSG_CUDA(cudaFuncSetAttribute(k_pmvT_lines<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, TSMEM));
     BSG_CUDA(cudaFuncSetAttribute(k_pmvT2<1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, T2SMEM));
     BSG_CUDA(cudaFuncSetAttribute(k_pmvT2<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, T2SMEM));
     BSG_CUDA(cudaFuncSetAttribute(k_pmvT2<2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, T2SMEM));
@@ -1612,10 +1734,13 @@ static int run_pmvT(bsg_view *v, const uint8_t *dig_raw, int plane, const uint8_
   if (g_timing) cudaEventRecord(g_ev0[g_ev_n % EV_POOL], s);
   if (!plane) {
     const int grid = a.nblocks * a.ksplit;
-    if (lines)
-      k_pmvT<0, true><<<grid, thr, TSMEM, s>>>(a);
-    else
-      k_pmvT<0, false><<<grid, thr, TSMEM, s>>>(a);
+    if (lines) {
+      k_pmvT_lines<0><<<grid, thr, TSMEM, s>>>(a);
+    } else {
+      CUtensorMap map;
+      BSG_TRY(make_map(&map, a.P, nc, a.stride, TLINES));
+      k_pmvT<0><<<grid, thr, TSMEM_TMA, s>>>(map, a);
+    }
   } else {
     // both planes in one pass: 32-byte strips per warp, twice the sample blocks
     a.nblocks = (int)((nbytes + T2BYTES - 1) / T2BYTES);
