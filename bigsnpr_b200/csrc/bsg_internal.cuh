@@ -240,5 +240,5 @@ struct bsg_view {
   int *d_row_gather = nullptr;   // [nr] position of each requested row in d_rows_unique
   int nru = 0;
   // scratch owned by the view (so device-pointer calls are allocation free)
-  bsg::DevBuf s_vec0, s_vec1, s_vec2, s_q0, s_q1, s_dig1, s_dig2, s_part, s_scal, s_full;
+  bsg::DevBuf s_vec0, s_vec1, s_q0, s_q1, s_dig1, s_dig2, s_part, s_scal, s_full;
 };

@@ -387,116 +387,26 @@ __device__ __forceinline__ void make_vals(int mode, const double *x, const doubl
   }
 }
 
-__global__ void k_scal_reset(Scal *sc) {
-  sc->maxabs[0] = sc->maxabs[1] = 0;
-  sc->nonfinite = 0;
-  sc->e[0] = sc->e[1] = 0;
-  sc->Y = 0;
-  sc->C = 0;
-  sc->sum_hi = sc->sum_lo = 0;
-}
-
-__global__ void k_maxabs(int mode, const double *__restrict__ x, const double *__restrict__ center,
-                         const double *__restrict__ scale, int len, Scal *sc) {
-  double m0 = 0, m1 = 0;
-  int bad = 0;
-  for (int k = blockIdx.x * blockDim.x + threadIdx.x; k < len; k += gridDim.x * blockDim.x) {
-    double v0, v1;
-    make_vals(mode, x, center, scale, k, v0, v1);
-    if (!isfinite(v0) || !isfinite(v1)) bad = 1;
-    m0 = fmax(m0, fabs(v0));
-    m1 = fmax(m1, fabs(v1));
-  }
-#pragma unroll
-  for (int o = 16; o; o >>= 1) {
-    m0 = fmax(m0, __shfl_xor_sync(0xffffffffu, m0, o));
-    m1 = fmax(m1, __shfl_xor_sync(0xffffffffu, m1, o));
-    bad |= __shfl_xor_sync(0xffffffffu, bad, o);
-  }
-  if ((threadIdx.x & 31) == 0) {
-    // non-negative doubles order like their bit patterns
-    atomicMax(reinterpret_cast<unsigned long long *>(&sc->maxabs[0]), (unsigned long long)__double_as_longlong(m0));
-    atomicMax(reinterpret_cast<unsigned long long *>(&sc->maxabs[1]), (unsigned long long)__double_as_longlong(m1));
-    if (bad) atomicOr(&sc->nonfinite, 1);
-  }
-}
-
-// e = 60 - exponent(maxabs) - headroom_bits, so that |sum of <= 2^headroom quantised values| < 2^60
-__global__ void k_pick_exp(Scal *sc, int headroom_bits) {
-  for (int p = 0; p < 2; p++) {
-    double m = sc->maxabs[p];
-    int ex = 0;
-    if (m > 0 && isfinite(m)) {
-      frexp(m, &ex);
-      sc->e[p] = 60 - ex - headroom_bits;
-    } else {
-      sc->e[p] = 0;
-    }
-  }
-}
-
-// Q[idx ? idx[k] : k] (+)= rint(v * 2^e).  With idx the destination is pre-zeroed and duplicates add
-// up in integers (order independent) -- the scatter side of `ind.row` / `ind.col` multisets.
-__global__ void k_quantise(int mode, const double *__restrict__ x, const double *__restrict__ center,
-                           const double *__restrict__ scale, int len, const int *__restrict__ idx, const Scal *sc,
-                           long long *__restrict__ Q0, long long *__restrict__ Q1) {
-  const int e0 = sc->e[0], e1 = sc->e[1];
-  const bool bad = sc->nonfinite != 0;
-  for (int k = blockIdx.x * blockDim.x + threadIdx.x; k < len; k += gridDim.x * blockDim.x) {
-    double v0, v1;
-    make_vals(mode, x, center, scale, k, v0, v1);
-    long long q0 = bad ? 0 : __double2ll_rn(scalbn(v0, e0));
-    long long q1 = (bad || !Q1) ? 0 : __double2ll_rn(scalbn(v1, e1));
-    if (idx) {
-      atomicAdd(reinterpret_cast<unsigned long long *>(Q0 + idx[k]), (unsigned long long)q0);
-      if (Q1) atomicAdd(reinterpret_cast<unsigned long long *>(Q1 + idx[k]), (unsigned long long)q1);
-    } else {
-      Q0[k] = q0;
-      if (Q1) Q1[k] = q1;
-    }
-  }
-}
-
-// digits: one thread per 16-byte unit (chunk, w, s, q) -> 16 int8 digits of slice s for the 16 codes of
-// word w of lane q (bytes 16q + 4w of the chunk for w < 4, bytes 64 + 16q + 4(w-4) for w >= 4), i.e. codes
-// t = (w < 4 ? 64 q + 16 w : 256 + 64 q + 16 (w - 4)) + 4 r + c, stored at byte c*4 + r  (see tile_stage).
-__global__ void k_digits(const long long *__restrict__ Q, int len, int nchunks, uint8_t *__restrict__ dig) {
-  int64_t total = (int64_t)nchunks * 256;
-  for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
-    int chunk = (int)(t >> 8), unit = (int)(t & 255);
-    int q = unit & 3, s = (unit >> 2) & 7, w = unit >> 5;
-    uint32_t out[4] = {0, 0, 0, 0};
-#pragma unroll
-    for (int c = 0; c < 4; c++) {
-#pragma unroll
-      for (int r = 0; r < 4; r++) {
-        int64_t k = (int64_t)chunk * CODES + (w < 4 ? 64 * q + 16 * w : 256 + 64 * q + 16 * (w - 4)) + 4 * r + c;
-        long long v = k < len ? Q[k] : 0;
-        // signed base-256 digit s: peel s digits
-        int d = 0;
-        for (int i = 0; i <= s; i++) {
-          d = (int)(signed char)(v & 0xFF);
-          v = (v - d) >> 8;
-        }
-        out[c] |= (uint32_t)(d & 0xFF) << (8 * r);
-      }
-    }
-    reinterpret_cast<uint4 *>(dig)[t] = make_uint4(out[0], out[1], out[2], out[3]);
-  }
-}
-
-// e = 60 - exponent(maxabs) - headroom_bits  ->  |sum of <= 2^hb quantised values| < 2^60
-__device__ __forceinline__ int pick_e(double m, int hb) {
+// e = bits - exponent(maxabs) - hb, so that |sum of <= 2^hb quantised values| < 2^bits.  bits = 60: one vector in 8
+// signed base-256 digits; bits = 30: one of two vectors sharing a pass in 4 digits (max 127 * (2^32 - 1) / 255).
+__device__ __forceinline__ int pick_e(double m, int hb, int bits) {
   int ex = 0;
   if (m > 0 && isfinite(m)) {
     frexp(m, &ex);
-    return 60 - ex - hb;
+    return bits - ex - hb;
   }
   return 0;
 }
 
-// Fused preparation, direct (identity index) path -- pass 1: max |v0|, max |v1|, finiteness and, for X.y with
-// scaling, the per-block partials of C = sum_k c_k z_k.  Fixed grid of SUMCZ_BLOCKS blocks.
+// the next signed base-256 digit of q (its low byte as int8); q keeps the exact rest (q - d) / 256
+__device__ __forceinline__ int peel(long long &q) {
+  const int d = (int)(signed char)(q & 0xFF);
+  q = (q - d) >> 8;
+  return d;
+}
+
+// pass 1 on every path: max |v0|, max |v1|, finiteness and, for X.y with scaling, the per-block partials of
+// C = sum_k c_k z_k.  Fixed grid of SUMCZ_BLOCKS blocks; one launch per vector.
 __global__ void k_prep1(int mode, const double *__restrict__ x, const double *__restrict__ center,
                         const double *__restrict__ scale, int len, int hb, Scal *sc) {
   __shared__ double sh[32];
@@ -518,6 +428,7 @@ __global__ void k_prep1(int mode, const double *__restrict__ x, const double *__
     cz += __shfl_xor_sync(0xffffffffu, cz, o);
   }
   if ((threadIdx.x & 31) == 0) {
+    // non-negative doubles order like their bit patterns
     atomicMax(reinterpret_cast<unsigned long long *>(&sc->maxabs[0]), (unsigned long long)__double_as_longlong(m0));
     atomicMax(reinterpret_cast<unsigned long long *>(&sc->maxabs[1]), (unsigned long long)__double_as_longlong(m1));
     if (bad) atomicOr(&sc->nonfinite, 1);
@@ -532,22 +443,52 @@ __global__ void k_prep1(int mode, const double *__restrict__ x, const double *__
   }
 }
 
-// pass 2: quantise and lay out the digits straight from the input vector (no Q array).  One thread per
-// 16-byte unit (chunk, w, s, q) as in k_digits; with two planes the thread writes both units.  want_sum: the
-// slice-0 threads also accumulate the exact integer sum of Q (Xt.y needs Y = sum y).
-__global__ void k_prep2(int mode, const double *__restrict__ x, const double *__restrict__ center,
-                        const double *__restrict__ scale, int len, int nchunks, Scal *sc, uint8_t *__restrict__ dig1,
-                        uint8_t *__restrict__ dig2, int want_sum, long long *__restrict__ qout = nullptr) {
-  const int e0 = pick_e(sc->maxabs[0], sc->hb), e1 = pick_e(sc->maxabs[1], sc->hb);
+// Scatter of an index multiset (`ind.row` / `ind.col`): Q[idx[k]] += rint(v * 2^e) into a pre-zeroed Q, so duplicates
+// add up in integers (order independent).  The exponents follow from what k_prep1 left in *sc.
+__global__ void k_quantise(int mode, const double *__restrict__ x, const double *__restrict__ center,
+                           const double *__restrict__ scale, int len, const int *__restrict__ idx, const Scal *sc, int bits,
+                           long long *__restrict__ Q0, long long *__restrict__ Q1) {
+  const int e0 = pick_e(sc->maxabs[0], sc->hb, bits), e1 = pick_e(sc->maxabs[1], sc->hb, bits);
   const bool bad = sc->nonfinite != 0;
+  for (int k = blockIdx.x * blockDim.x + threadIdx.x; k < len; k += gridDim.x * blockDim.x) {
+    double v0, v1;
+    make_vals(mode, x, center, scale, k, v0, v1);
+    const long long q0 = bad ? 0 : __double2ll_rn(scalbn(v0, e0));
+    atomicAdd(reinterpret_cast<unsigned long long *>(Q0 + idx[k]), (unsigned long long)q0);
+    if (Q1) {
+      const long long q1 = bad ? 0 : __double2ll_rn(scalbn(v1, e1));
+      atomicAdd(reinterpret_cast<unsigned long long *>(Q1 + idx[k]), (unsigned long long)q1);
+    }
+  }
+}
+
+// pass 2, the k_pmv digit layout: one thread per (chunk, w, q).  Code t = (w < 4 ? 64 q + 16 w : 256 + 64 q + 16 (w - 4))
+// + 4 r + c of a chunk (word w of lane q in k_pmv) goes to byte c * 4 + r of the 16-byte unit (w * 8 + slice) * 4 + q.
+// The values come straight from the vector(s) (Q0 == null: identity selection, len = the staged length) or from what
+// k_quantise scattered into Q0 / Q1.  NV = 1: one vector, 8 slices in dig1, its second value v1 in dig2 (if given).
+// NV = 2: vectors x and xb (scalars sc[0] / sc[1]; xb may be null), slices 0..3 and 4..7 of dig1.  want_sum: the exact
+// integer sum of the raw-plane Q (Xt.y needs Y = sum y); qout: the raw-plane Q by position.
+template <int NV>
+__global__ void k_prep2(int mode, const double *__restrict__ x, const double *__restrict__ center,
+                        const double *__restrict__ scale, const double *__restrict__ xb, int len, int nchunks, Scal *sc,
+                        const long long *__restrict__ Q0, const long long *__restrict__ Q1, uint8_t *__restrict__ dig1,
+                        uint8_t *__restrict__ dig2, int want_sum, long long *__restrict__ qout) {
+  constexpr int NS = 8 / NV, BITS = NV == 1 ? 60 : 30;
+  // stream a = raw plane of the (first) vector, stream b = its second plane (NV = 1) or the raw plane of xb (NV = 2)
+  const Scal &sa = sc[0], &sb = sc[NV - 1];
+  const int ea = pick_e(sa.maxabs[0], sa.hb, BITS), eb = pick_e(sb.maxabs[NV == 1 ? 1 : 0], sb.hb, BITS);
+  const bool bada = sa.nonfinite != 0, badb = sb.nonfinite != 0;
   if (blockIdx.x == 0 && threadIdx.x == 0) {
-    sc->e[0] = e0;
-    sc->e[1] = e1;
+    for (int v = 0; v < NV; v++) {
+      sc[v].e[0] = pick_e(sc[v].maxabs[0], sc[v].hb, BITS);
+      sc[v].e[1] = pick_e(sc[v].maxabs[1], sc[v].hb, BITS);
+    }
   }
   long long hi = 0, lo = 0;
-  // 2^e as a double when it is a normal number (always, unless the vector is denormal-small or huge)
-  const bool fast0 = e0 > -1000 && e0 < 1000, fast1 = e1 > -1000 && e1 < 1000;
-  const double f0 = fast0 ? scalbn(1.0, e0) : 0.0, f1 = fast1 ? scalbn(1.0, e1) : 0.0;
+  // 2^e as a double when it is a normal number (always, unless the vector is denormal-small or huge); v * 2^e is then
+  // the same double as scalbn(v, e)
+  const bool fasta = ea > -1000 && ea < 1000, fastb = eb > -1000 && eb < 1000;
+  const double fa = fasta ? scalbn(1.0, ea) : 0.0, fb = fastb ? scalbn(1.0, eb) : 0.0;
   int64_t total = (int64_t)nchunks * 32;  // (chunk, w, q)
   for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
     const int chunk = (int)(t >> 5), wq = (int)(t & 31);
@@ -563,11 +504,22 @@ __global__ void k_prep2(int mode, const double *__restrict__ x, const double *__
       for (int r = 0; r < 4; r++) {
         int64_t k = (int64_t)chunk * CODES + (w < 4 ? 64 * q + 16 * w : 256 + 64 * q + 16 * (w - 4)) + 4 * r + c;
         long long qa = 0, qb = 0;
-        if (k < len && !bad) {
-          double v0, v1;
-          make_vals(mode, x, center, scale, (int)k, v0, v1);
-          qa = __double2ll_rn(fast0 ? v0 * f0 : scalbn(v0, e0));
-          if (dig2) qb = __double2ll_rn(fast1 ? v1 * f1 : scalbn(v1, e1));
+        if (k < len) {
+          if (Q0) {
+            qa = Q0[k];
+            if (Q1) qb = Q1[k];
+          } else {
+            double v0, v1;
+            if (!bada) {
+              make_vals(mode, x, center, scale, (int)k, v0, v1);
+              qa = __double2ll_rn(fasta ? v0 * fa : scalbn(v0, ea));
+              if (NV == 1 && dig2) qb = __double2ll_rn(fastb ? v1 * fb : scalbn(v1, eb));
+            }
+            if (NV == 2 && xb && !badb) {
+              make_vals(mode, xb, center, scale, (int)k, v0, v1);
+              qb = __double2ll_rn(fastb ? v0 * fb : scalbn(v0, eb));
+            }
+          }
         }
         if (want_sum) {
           hi += qa >> 32;
@@ -575,15 +527,12 @@ __global__ void k_prep2(int mode, const double *__restrict__ x, const double *__
         }
         if (qout && k < len) qout[k] = qa;  // the quantised raw-plane vector (sparse missing-value correction)
 #pragma unroll
-        for (int sl = 0; sl < 8; sl++) {
-          int d = (int)(signed char)(qa & 0xFF);
-          qa = (qa - d) >> 8;
-          o1[sl][c] |= (uint32_t)(d & 0xFF) << (8 * r);
-          if (dig2) {
-            int d2 = (int)(signed char)(qb & 0xFF);
-            qb = (qb - d2) >> 8;
-            o2[sl][c] |= (uint32_t)(d2 & 0xFF) << (8 * r);
-          }
+        for (int sl = 0; sl < NS; sl++) {
+          o1[sl][c] |= (uint32_t)(peel(qa) & 0xFF) << (8 * r);
+          if (NV == 2)
+            o1[NS + sl][c] |= (uint32_t)(peel(qb) & 0xFF) << (8 * r);
+          else if (dig2)
+            o2[sl][c] |= (uint32_t)(peel(qb) & 0xFF) << (8 * r);
         }
       }
     }
@@ -591,7 +540,7 @@ __global__ void k_prep2(int mode, const double *__restrict__ x, const double *__
     for (int sl = 0; sl < 8; sl++) {
       const int64_t unit = (int64_t)chunk * 256 + (w * 8 + sl) * 4 + q;
       reinterpret_cast<uint4 *>(dig1)[unit] = make_uint4(o1[sl][0], o1[sl][1], o1[sl][2], o1[sl][3]);
-      if (dig2) reinterpret_cast<uint4 *>(dig2)[unit] = make_uint4(o2[sl][0], o2[sl][1], o2[sl][2], o2[sl][3]);
+      if (NV == 1 && dig2) reinterpret_cast<uint4 *>(dig2)[unit] = make_uint4(o2[sl][0], o2[sl][1], o2[sl][2], o2[sl][3]);
     }
   }
   if (want_sum) {
@@ -607,49 +556,10 @@ __global__ void k_prep2(int mode, const double *__restrict__ x, const double *__
   }
 }
 
-// exact integer sum of Q (split in 32-bit halves, integer atomics: order independent); Y is formed from
-// (sum_hi, sum_lo) in the finish kernel.
-__global__ void k_sum_q(const long long *__restrict__ Q, int len, Scal *sc) {
-  long long hi = 0, lo = 0;
-  for (int k = blockIdx.x * blockDim.x + threadIdx.x; k < len; k += gridDim.x * blockDim.x) {
-    long long v = Q[k];
-    hi += v >> 32;
-    lo += (long long)(unsigned int)(v & 0xFFFFFFFFll);
-  }
-#pragma unroll
-  for (int o = 16; o; o >>= 1) {
-    hi += __shfl_xor_sync(0xffffffffu, hi, o);
-    lo += __shfl_xor_sync(0xffffffffu, lo, o);
-  }
-  if ((threadIdx.x & 31) == 0) {
-    atomicAdd(reinterpret_cast<unsigned long long *>(&sc->sum_hi), (unsigned long long)hi);
-    atomicAdd(reinterpret_cast<unsigned long long *>(&sc->sum_lo), (unsigned long long)lo);
-  }
-}
-
-// C = sum_k c_k * (x_k / s_k): per-block partial sums with a fixed-shape tree, written to cpart[block];
-// the finish kernel adds the SUMCZ_BLOCKS partials in index order -> deterministic.
-__global__ void k_sum_cz(const double *__restrict__ x, const double *__restrict__ center,
-                         const double *__restrict__ scale, int len, double *__restrict__ cpart) {
-  __shared__ double sh[32];
-  double acc = 0;
-  for (int k = blockIdx.x * blockDim.x + threadIdx.x; k < len; k += gridDim.x * blockDim.x)
-    acc += center[k] * (x[k] / scale[k]);
-#pragma unroll
-  for (int o = 16; o; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = acc;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double t = 0;
-    for (int w = 0; w < (int)(blockDim.x >> 5); w++) t += sh[w];
-    cpart[blockIdx.x] = t;
-  }
-}
-
 // Xt.y:  out_j = ((R - 3N) - c_j (Y - N)) / s_j        (bedAccScaled semantics, src/bed-acc.h:98-111)
-__global__ void k_finish_cprod(const long long *__restrict__ part, int ksplit, int64_t nlines_pad, int nlines,
-                               const Scal *sc, const double *__restrict__ center, const double *__restrict__ scale,
-                               int use_na, double *__restrict__ out) {
+__global__ void k_finish_cprod(const long long *__restrict__ part, int nlines, const Scal *sc,
+                               const double *__restrict__ center, const double *__restrict__ scale, int use_na,
+                               double *__restrict__ out) {
   int j = blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= nlines) return;
   if (sc->nonfinite) {
@@ -657,8 +567,8 @@ __global__ void k_finish_cprod(const long long *__restrict__ part, int ksplit, i
     return;
   }
   const int e = sc->e[0];
-  double G = combine8(part, j, 1, use_na ? -3 : 0, e);  // R - 3N, exact
-  double N = use_na ? combine8(part, j, 0, 1, e) : 0.0;
+  double G = combine<8>(part, j, 0, 1, use_na ? -3 : 0, e);  // R - 3N, exact
+  double N = use_na ? combine<8>(part, j, 0, 0, 1, e) : 0.0;
   if (center) {
     const double Y = scalbn((double)sc->sum_hi, 32 - e) + scalbn((double)sc->sum_lo, -e);
     out[j] = (G - center[j] * (Y - N)) / scale[j];
@@ -667,10 +577,9 @@ __global__ void k_finish_cprod(const long long *__restrict__ part, int ksplit, i
   }
 }
 
-// X.y:  full_l = R + Nw - C   with Nw the NA-plane sum against w = (c - 3) z;  without scaling
-// full_l = R - 3 N.   out[i] = full[gather[i]].
-__global__ void k_finish_prod(const long long *__restrict__ part, int ksplit, int64_t nlines_pad, int nlines,
-                              const Scal *sc, int has_scaling, int use_na, double *__restrict__ full) {
+// X.y (finish_prod_value):  full_l = R + Nw - C, or R - 3 N without scaling.   out[i] = full[gather[i]].
+__global__ void k_finish_prod(const long long *__restrict__ part, int nlines, const Scal *sc, int has_scaling, int use_na,
+                              double *__restrict__ full) {
   int l = blockIdx.x * blockDim.x + threadIdx.x;
   if (l >= nlines) return;
   full[l] = finish_prod_value(part, l, sc, has_scaling, use_na);
@@ -688,8 +597,8 @@ __global__ void k_finish_planes(const long long *__restrict__ part, int nlines, 
     if (fullB) fullB[l] = nan("");
     return;
   }
-  const double R = combine8(part, l, 1, 0, sc->e[0]);
-  const double P = have_p ? combine8(part, l, 0, 1, sc->e[p_same ? 0 : 1]) : 0.0;
+  const double R = combine<8>(part, l, 0, 1, 0, sc->e[0]);
+  const double P = have_p ? combine<8>(part, l, 0, 0, 1, sc->e[p_same ? 0 : 1]) : 0.0;
   full[l] = (cR * R + cP * P) + add0;
   if (fullB) fullB[l] = cRb * R + cPb * P;
 }
@@ -719,6 +628,56 @@ static int hb_bits(int maxmult) {
   int b = 0;
   while ((1 << b) < maxmult) b++;
   return b;
+}
+
+// Digits of the k_pmv layout for a vector over the selected columns (dir 0: lines = samples of copy B) or over the
+// selected samples (dir 1: lines = SNP columns of copy A).  nv = 1: one vector of make_vals(mode, x, p1, p2), 60 bits,
+// its second value into s_dig2 when `two`.  nv = 2: the vectors x and xb (mode 0, 30 bits each, 4 + 4 slices of s_dig1;
+// xb may be null), scalars in sc[0] / sc[1].  An identity selection is laid out straight from the vector; an index
+// multiset is first scattered into s_q0 / s_q1.  want_sum: the exact sum of Q into sc->sum_hi / sum_lo; keep_q: s_q0
+// ends up holding the raw-plane Q by position.
+static int prep_pmv(bsg_view *v, int dir, int mode, const double *x, const double *p1, const double *p2, int nv,
+                    const double *xb, bool two, bool want_sum, bool keep_q, cudaStream_t s) {
+  bsg_bed *h = v->h;
+  const bool cols = dir == 0;
+  const int L = cols ? h->m : h->n, len = cols ? v->nc : v->nr;
+  const int *idx = (cols ? v->col_identity : v->row_identity) ? nullptr : (cols ? v->d_col : v->d_row);
+  const int hb = hb_bits(cols ? v->col_maxmult : v->row_maxmult);
+  const int nchunks = (int)((cols ? h->strideB : h->strideA) / SEG);
+  Scal *sc = v->s_scal.as<Scal>();
+  BSG_TRY(v->s_dig1.ensure((size_t)nchunks * DIG));
+  if (two) BSG_TRY(v->s_dig2.ensure((size_t)nchunks * DIG));
+  uint8_t *dig1 = v->s_dig1.as<uint8_t>(), *dig2 = two ? v->s_dig2.as<uint8_t>() : nullptr;
+  long long *Q0 = nullptr, *Q1 = nullptr;
+  if (idx || keep_q) {
+    BSG_TRY(v->s_q0.ensure((size_t)L * sizeof(long long)));
+    Q0 = v->s_q0.as<long long>();
+  }
+  if (idx && (two || xb)) {
+    BSG_TRY(v->s_q1.ensure((size_t)L * sizeof(long long)));
+    Q1 = v->s_q1.as<long long>();
+  }
+  BSG_CUDA(cudaMemsetAsync(sc, 0, nv * sizeof(Scal), s));
+  k_prep1<<<SUMCZ_BLOCKS, 256, 0, s>>>(mode, x, p1, p2, len, hb, sc);
+  if (xb) k_prep1<<<SUMCZ_BLOCKS, 256, 0, s>>>(mode, xb, p1, p2, len, hb, sc + 1);
+  count_launch(xb ? 2 : 1);
+  if (idx) {
+    const int bits = nv == 1 ? 60 : 30;
+    BSG_CUDA(cudaMemsetAsync(Q0, 0, (size_t)L * sizeof(long long), s));
+    if (Q1) BSG_CUDA(cudaMemsetAsync(Q1, 0, (size_t)L * sizeof(long long), s));
+    k_quantise<<<launch_cap(len, 256, 592), 256, 0, s>>>(mode, x, p1, p2, len, idx, sc, bits, Q0, nv == 1 ? Q1 : nullptr);
+    if (xb) k_quantise<<<launch_cap(len, 256, 592), 256, 0, s>>>(mode, xb, p1, p2, len, idx, sc + 1, bits, Q1, nullptr);
+    count_launch(xb ? 2 : 1);
+  }
+  const int grid = launch_cap((int64_t)nchunks * 32, 128, 1184);
+  const long long *src0 = idx ? Q0 : nullptr;
+  if (nv == 1)
+    k_prep2<1><<<grid, 128, 0, s>>>(mode, x, p1, p2, nullptr, L, nchunks, sc, src0, Q1, dig1, dig2, want_sum,
+                                    idx ? nullptr : Q0);
+  else
+    k_prep2<2><<<grid, 128, 0, s>>>(mode, x, p1, p2, xb, L, nchunks, sc, src0, Q1, dig1, nullptr, want_sum, nullptr);
+  count_launch();
+  return BSG_OK;
 }
 
 // shared launcher of the tensor-pipe kernel + scratch sizing
@@ -1292,112 +1251,59 @@ __global__ void __launch_bounds__(TWARPS * 32, 2) k_pmvT2(const TArgs a, const u
         }
 }
 
-// digits of the quantised vector(s) in step order: dig[(t / 32) * 256 + slice * 32 + (t % 32)]
-__global__ void k_quantT(int mode, const double *__restrict__ x, const double *__restrict__ center,
-                         const double *__restrict__ scale, int len, int len_pad, const pmv::Scal *sc,
-                         uint8_t *__restrict__ dig1, uint8_t *__restrict__ dig2, const int *__restrict__ lines = nullptr,
-                         long long *__restrict__ qna_full = nullptr, int na_second = 0, pmv::Scal *pick = nullptr) {
-  // pick: the exponents are derived here from the maxima k_prep1 left in *sc (and published for the finish kernels)
-  const int e0 = pick ? pmv::pick_e(sc->maxabs[0], sc->hb) : sc->e[0], e1 = pick ? pmv::pick_e(sc->maxabs[1], sc->hb) : sc->e[1];
-  if (pick && blockIdx.x == 0 && threadIdx.x == 0) {
-    pick->e[0] = e0;
-    pick->e[1] = e1;
-  }
-  const bool bad = sc->nonfinite != 0;
-  for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < len_pad; t += gridDim.x * blockDim.x) {
-    long long q0 = 0, q1 = 0;
-    if (t < len && !bad) {
-      double v0, v1;
-      pmv::make_vals(mode, x, center, scale, t, v0, v1);
-      q0 = __double2ll_rn(scalbn(v0, e0));
-      if (dig2 || na_second) q1 = __double2ll_rn(scalbn(v1, e1));
-      if (qna_full)  // missing-value vector by physical line (duplicates of a column add up)
-        atomicAdd(reinterpret_cast<unsigned long long *>(qna_full + (lines ? lines[t] : t)),
-                  (unsigned long long)(na_second ? q1 : q0));
-    }
-    const int64_t base = (int64_t)(t >> 5) * 256 + (t & 31);
-#pragma unroll
-    for (int sl = 0; sl < 8; sl++) {
-      int d = (int)(signed char)(q0 & 0xFF);
-      q0 = (q0 - d) >> 8;
-      dig1[base + sl * 32] = (uint8_t)d;
-      if (dig2) {
-        int d2 = (int)(signed char)(q1 & 0xFF);
-        q1 = (q1 - d2) >> 8;
-        dig2[base + sl * 32] = (uint8_t)d2;
-      }
-    }
-  }
-}
-
-// ---- two vectors per pass (PCA projection, bsg_prod_and_rowsumssq) ---------------------------------------------------
+// ---- two vectors per pass (PCA projection, bsg_prod_and_rowsumssq; multLinReg through k_pmv) ------------------------
 // An IMMA always produces 8 columns; with the full 61-bit fixed point all 8 are digit slices of ONE vector.  For the K
 // columns of a projection the vectors are quantised to 30 bits instead (4 signed base-256 digits, |Q| < 2^30 relative to
 // the largest entry of the vector: ~1e-9 of the result, three orders inside the 1e-6 contract) and TWO vectors share a
 // pass: columns 0..3 = vector 1, 4..7 = vector 2.  Same kernels, same bytes read, twice the vectors.
-__global__ void k_pick_exp_pair(pmv::Scal *sc, int headroom_bits) {
-  const int v = threadIdx.x >> 1, p = threadIdx.x & 1;  // 4 threads: (vector, plane)
-  if (threadIdx.x >= 4) return;
-  const double m = sc[v].maxabs[p];
-  int ex = 0;
-  if (m > 0 && isfinite(m)) {
-    frexp(m, &ex);
-    sc[v].e[p] = 30 - ex - headroom_bits;  // |Q| < 2^30 fits 4 signed base-256 digits (max 127 * (2^32 - 1) / 255)
-  } else {
-    sc[v].e[p] = 0;
-  }
-}
 
-// dig[(t / 32) * 256 + slice * 32 + (t % 32)], slices 0..3 = vector 1, 4..7 = vector 2; dig2 = the (c - 3) z plane
-__global__ void k_quantT_pair(int mode, const double *__restrict__ xa, const double *__restrict__ xb,
-                              const double *__restrict__ center, const double *__restrict__ scale, int len, int len_pad,
-                              const pmv::Scal *sc, uint8_t *__restrict__ dig1, uint8_t *__restrict__ dig2) {
-  const int e0a = sc[0].e[0], e1a = sc[0].e[1], e0b = sc[1].e[0], e1b = sc[1].e[1];
-  const bool bada = sc[0].nonfinite != 0, badb = sc[1].nonfinite != 0;
-  for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < len_pad; t += gridDim.x * blockDim.x) {
-    long long q[2][2] = {{0, 0}, {0, 0}};  // [vector][plane]
-    if (t < len) {
-      double v0, v1;
-      if (!bada) {
-        pmv::make_vals(mode, xa, center, scale, t, v0, v1);
-        q[0][0] = __double2ll_rn(scalbn(v0, e0a));
-        if (dig2) q[0][1] = __double2ll_rn(scalbn(v1, e1a));
-      }
-      if (xb && !badb) {
-        pmv::make_vals(mode, xb, center, scale, t, v0, v1);
-        q[1][0] = __double2ll_rn(scalbn(v0, e0b));
-        if (dig2) q[1][1] = __double2ll_rn(scalbn(v1, e1b));
-      }
+// Digits of the quantised vector(s) in step order: dig[(t / 32) * 256 + slice * 32 + (t % 32)].  The exponents are
+// derived here from the maxima k_prep1 left in sc[] and published for the finish kernels.  NV = 1: one vector, 8 slices,
+// v1 into dig2 (if given).  NV = 2: vectors x and xb (sc[0] / sc[1]; xb may be null), slices 0..3 and 4..7, the v1 of
+// each into the same slices of dig2.  qna_full: the missing-value vector (v1 if na_second, else v0) by physical line,
+// duplicates of a column adding up.
+template <int NV>
+__global__ void k_quantT(int mode, const double *__restrict__ x, const double *__restrict__ xb,
+                         const double *__restrict__ center, const double *__restrict__ scale, int len, int len_pad,
+                         pmv::Scal *sc, uint8_t *__restrict__ dig1, uint8_t *__restrict__ dig2,
+                         const int *__restrict__ lines, long long *__restrict__ qna_full, int na_second) {
+  constexpr int NS = 8 / NV, BITS = NV == 1 ? 60 : 30;
+  int e[NV][2];
+  bool bad[NV];
+#pragma unroll
+  for (int v = 0; v < NV; v++) {
+    e[v][0] = pmv::pick_e(sc[v].maxabs[0], sc[v].hb, BITS);
+    e[v][1] = pmv::pick_e(sc[v].maxabs[1], sc[v].hb, BITS);
+    bad[v] = sc[v].nonfinite != 0;
+  }
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+#pragma unroll
+    for (int v = 0; v < NV; v++) {
+      sc[v].e[0] = e[v][0];
+      sc[v].e[1] = e[v][1];
     }
+  }
+  for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < len_pad; t += gridDim.x * blockDim.x) {
     const int64_t base = (int64_t)(t >> 5) * 256 + (t & 31);
 #pragma unroll
-    for (int vv = 0; vv < 2; vv++)
-#pragma unroll
-      for (int sl = 0; sl < 4; sl++) {
-        int d = (int)(signed char)(q[vv][0] & 0xFF);
-        q[vv][0] = (q[vv][0] - d) >> 8;
-        dig1[base + (4 * vv + sl) * 32] = (uint8_t)d;
-        if (dig2) {
-          int d2 = (int)(signed char)(q[vv][1] & 0xFF);
-          q[vv][1] = (q[vv][1] - d2) >> 8;
-          dig2[base + (4 * vv + sl) * 32] = (uint8_t)d2;
-        }
+    for (int v = 0; v < NV; v++) {
+      long long q0 = 0, q1 = 0;
+      if (t < len && (v == 0 || xb) && !bad[v]) {
+        double v0, v1;
+        pmv::make_vals(mode, v ? xb : x, center, scale, t, v0, v1);
+        q0 = __double2ll_rn(scalbn(v0, e[v][0]));
+        if (dig2 || na_second) q1 = __double2ll_rn(scalbn(v1, e[v][1]));
+        if (qna_full)
+          atomicAdd(reinterpret_cast<unsigned long long *>(qna_full + (lines ? lines[t] : t)),
+                    (unsigned long long)(na_second ? q1 : q0));
       }
-  }
-}
-
-// (raw-plane * c0 + NA-plane * c1) over the 4 slices of vector vv
-__device__ __forceinline__ double combine4(const long long *__restrict__ part, int64_t line, int vv, int c0, int c1, int e) {
-  const long long *p = part + line * 16 + 4 * vv;
-  double acc = 0;
 #pragma unroll
-  for (int s = 3; s >= 0; s--) {
-    long long v = 0;
-    if (c0) v += c0 * p[s];
-    if (c1) v += c1 * p[8 + s];
-    acc += scalbn((double)v, 8 * s - e);
+      for (int sl = 0; sl < NS; sl++) {
+        dig1[base + (NS * v + sl) * 32] = (uint8_t)pmv::peel(q0);
+        if (dig2) dig2[base + (NS * v + sl) * 32] = (uint8_t)pmv::peel(q1);
+      }
+    }
   }
-  return acc;
 }
 
 __global__ void k_finish_prod_pair(const long long *__restrict__ part, int nlines, const pmv::Scal *sc, int has_scaling,
@@ -1407,49 +1313,7 @@ __global__ void k_finish_prod_pair(const long long *__restrict__ part, int nline
 #pragma unroll
   for (int vv = 0; vv < 2; vv++) {
     double *out = vv ? out2 : out1;
-    if (!out) continue;
-    double r;
-    if (sc[vv].nonfinite) {
-      r = nan("");
-    } else if (has_scaling) {
-      double C = 0;
-      for (int b = 0; b < pmv::SUMCZ_BLOCKS; b++) C += sc[vv].cpart[b];
-      const double R = combine4(part, l, vv, 1, 0, sc[vv].e[0]);
-      const double Nw = use_na ? combine4(part, l, vv, 0, 1, sc[vv].e[1]) : 0.0;
-      r = (R + Nw) - C;
-    } else {
-      r = combine4(part, l, vv, 1, use_na ? -3 : 0, sc[vv].e[0]);
-    }
-    out[l] = r;
-  }
-}
-
-// Two vectors per pass through k_pmv (lines = SNP columns, vectors over the samples: multLinReg).  Digit layout of
-// k_digits, slices 0..3 = 30-bit vector 1 (Qa), 4..7 = vector 2 (Qb).
-__global__ void k_digits_pair(const long long *__restrict__ Qa, const long long *__restrict__ Qb, int len, int nchunks,
-                              uint8_t *__restrict__ dig) {
-  const int64_t total = (int64_t)nchunks * 256;
-  for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
-    const int chunk = (int)(t >> 8), unit = (int)(t & 255);
-    const int q = unit & 3, s = (unit >> 2) & 7, w = unit >> 5;
-    const long long *Q = s < 4 ? Qa : Qb;
-    const int sd = s & 3;
-    uint32_t out[4] = {0, 0, 0, 0};
-#pragma unroll
-    for (int c = 0; c < 4; c++) {
-#pragma unroll
-      for (int r = 0; r < 4; r++) {
-        const int64_t k = (int64_t)chunk * pmv::CODES + (w < 4 ? 64 * q + 16 * w : 256 + 64 * q + 16 * (w - 4)) + 4 * r + c;
-        long long v = (Q && k < len) ? Q[k] : 0;
-        int d = 0;
-        for (int i = 0; i <= sd; i++) {
-          d = (int)(signed char)(v & 0xFF);
-          v = (v - d) >> 8;
-        }
-        out[c] |= (uint32_t)(d & 0xFF) << (8 * r);
-      }
-    }
-    reinterpret_cast<uint4 *>(dig)[t] = make_uint4(out[0], out[1], out[2], out[3]);
+    if (out) out[l] = pmv::finish_prod_value<4>(part, l, sc + vv, has_scaling, use_na, 4 * vv);
   }
 }
 
@@ -1472,8 +1336,8 @@ __global__ void k_finish_planes_pair(const long long *__restrict__ part, int nli
       if (c.outB) c.outB[l] = nan("");
       continue;
     }
-    const double R = combine4(part, l, vv, 1, 0, sc[vv].e[0]);
-    const double P = have_p ? combine4(part, l, vv, 0, 1, sc[vv].e[0]) : 0.0;
+    const double R = pmv::combine<4>(part, l, 4 * vv, 1, 0, sc[vv].e[0]);
+    const double P = have_p ? pmv::combine<4>(part, l, 4 * vv, 0, 1, sc[vv].e[0]) : 0.0;
     c.out[l] = c.cR * R + c.cP * P;
     if (c.outB) c.outB[l] = c.cRb * R + c.cPb * P;
   }
@@ -1600,8 +1464,8 @@ void bsg_view_destroy(bsg_view *v) {
   void *ptrs[] = {v->d_row, v->d_col, v->d_center, v->d_scale, v->d_rows_unique, v->d_row_gather};
   for (void *p : ptrs)
     if (p) cudaFree(p);
-  DevBuf *bufs[] = {&v->s_vec0, &v->s_vec1, &v->s_vec2, &v->s_q0, &v->s_q1, &v->s_dig1,
-                    &v->s_dig2, &v->s_part, &v->s_scal, &v->s_full};
+  DevBuf *bufs[] = {&v->s_vec0, &v->s_vec1, &v->s_q0, &v->s_q1, &v->s_dig1, &v->s_dig2, &v->s_part, &v->s_scal,
+                    &v->s_full};
   for (DevBuf *b : bufs) b->release();
   delete v;
 }
@@ -1617,38 +1481,14 @@ int bsg_view_cprodvec_dev(bsg_view *v, const double *x_dev, double *out_dev, voi
   if (v->nc == 0) return BSG_OK;
   using namespace pmv;
   Scal *sc = v->s_scal.as<Scal>();
-  const int n = h->n;
-  int nchunks = (int)(h->strideA / SEG);
-  BSG_TRY(v->s_q0.ensure((size_t)n * sizeof(long long)));
-  BSG_TRY(v->s_dig1.ensure((size_t)nchunks * DIG));
-  long long *Q = v->s_q0.as<long long>();
-  const int hb = hb_bits(v->row_maxmult);
   // few missing values: the kernel runs in its no-missing mode and the N plane comes from the per-SNP lists
   const bool lists = h->has_na && na_ell_ready(h);
-  if (v->row_identity) {
-    // direct path: memset + 2 kernels
-    BSG_CUDA(cudaMemsetAsync(sc, 0, sizeof(Scal), s));
-    k_prep1<<<SUMCZ_BLOCKS, 256, 0, s>>>(0, x_dev, nullptr, nullptr, v->nr, hb, sc);
-    k_prep2<<<launch_cap((int64_t)nchunks * 32, 128, 1184), 128, 0, s>>>(0, x_dev, nullptr, nullptr, n, nchunks, sc,
-                                                                          v->s_dig1.as<uint8_t>(), nullptr, 1,
-                                                                          lists ? Q : nullptr);
-    count_launch(2);
-  } else {
-    k_scal_reset<<<1, 1, 0, s>>>(sc);
-    k_maxabs<<<launch_cap(v->nr, 256, 592), 256, 0, s>>>(0, x_dev, nullptr, nullptr, v->nr, sc);
-    k_pick_exp<<<1, 1, 0, s>>>(sc, hb);
-    BSG_CUDA(cudaMemsetAsync(Q, 0, (size_t)n * sizeof(long long), s));
-    k_quantise<<<launch_cap(v->nr, 256, 592), 256, 0, s>>>(0, x_dev, nullptr, nullptr, v->nr, v->d_row, sc, Q, nullptr);
-    k_digits<<<launch_cap((int64_t)nchunks * 256, 256, 1184), 256, 0, s>>>(Q, n, nchunks, v->s_dig1.as<uint8_t>());
-    k_sum_q<<<launch_cap(n, 256, 296), 256, 0, s>>>(Q, n, sc);
-    count_launch(6);
-  }
+  BSG_TRY(prep_pmv(v, 1, 0, x_dev, nullptr, nullptr, 1, nullptr, false, true, lists, s));
   Args a;
-  BSG_TRY(run_pmv(v, h->A, h->strideA, n, v->d_col, v->nc, v->s_dig1.as<uint8_t>(), nullptr, h->naA,
+  BSG_TRY(run_pmv(v, h->A, h->strideA, h->n, v->d_col, v->nc, v->s_dig1.as<uint8_t>(), nullptr, h->naA,
                   lists ? 0 : h->has_na, &a, s));
-  if (lists) BSG_TRY(na_ell_correction(h, 1, v->d_col, v->nc, Q, a.part, s));
-  k_finish_cprod<<<(v->nc + 255) / 256, 256, 0, s>>>(a.part, a.ksplit, a.nlines_pad, v->nc, sc, v->d_center, v->d_scale,
-                                                      h->has_na, out_dev);
+  if (lists) BSG_TRY(na_ell_correction(h, 1, v->d_col, v->nc, v->s_q0.as<long long>(), a.part, s));
+  k_finish_cprod<<<(v->nc + 255) / 256, 256, 0, s>>>(a.part, v->nc, sc, v->d_center, v->d_scale, h->has_na, out_dev);
   count_launch();
   BSG_CUDA(cudaGetLastError());
   return BSG_OK;
@@ -1769,9 +1609,11 @@ static int run_pmvT(bsg_view *v, const uint8_t *dig_raw, int plane, const uint8_
   return BSG_OK;
 }
 
-// digit blocks of one or two vectors over the selected columns, in k_pmvT's step order
-static int prep_T(bsg_view *v, int mode, const double *x, const double *p1, const double *p2, bool two, cudaStream_t s,
-                  long long *qna_full = nullptr, int na_second = 0) {
+// Digit blocks over the selected columns in k_pmvT's step order.  nv = 1: one vector of make_vals(mode, x, p1, p2),
+// 60 bits, its second value into s_dig2 when `two`.  nv = 2: the vectors x and xb (30 bits each, 4 + 4 slices; xb may
+// be null), scalars in sc[0] / sc[1].  k_prep1 also leaves the block partials of C = sum c z (mode 1).
+static int prep_T(bsg_view *v, int mode, const double *x, const double *p1, const double *p2, int nv, const double *xb,
+                  bool two, cudaStream_t s, long long *qna_full = nullptr, int na_second = 0) {
   using namespace pmv;
   using namespace pmvt;
   Scal *sc = v->s_scal.as<Scal>();
@@ -1779,14 +1621,17 @@ static int prep_T(bsg_view *v, int mode, const double *x, const double *p1, cons
   const int nsteps = (nc + TLINES - 1) / TLINES;
   BSG_TRY(v->s_dig1.ensure((size_t)std::max(nsteps, 1) * 256));
   if (two) BSG_TRY(v->s_dig2.ensure((size_t)std::max(nsteps, 1) * 256));
-  // memset + 2 kernels: maxima, finiteness and (mode 1) the block partials of C = sum c z in one pass over the vector,
-  // then quantisation + digits with the exponents picked per block from the maxima
-  BSG_CUDA(cudaMemsetAsync(sc, 0, sizeof(Scal), s));
+  uint8_t *dig1 = v->s_dig1.as<uint8_t>(), *dig2 = two ? v->s_dig2.as<uint8_t>() : nullptr;
+  BSG_CUDA(cudaMemsetAsync(sc, 0, nv * sizeof(Scal), s));
   k_prep1<<<SUMCZ_BLOCKS, 256, 0, s>>>(mode, x, p1, p2, nc, 0, sc);
-  k_quantT<<<launch_cap((int64_t)std::max(nsteps, 1) * TLINES, 256, 1184), 256, 0, s>>>(
-      mode, x, p1, p2, nc, nsteps * TLINES, sc, v->s_dig1.as<uint8_t>(), two ? v->s_dig2.as<uint8_t>() : nullptr, v->d_col,
-      qna_full, na_second, sc);
-  count_launch(2);
+  if (xb) k_prep1<<<SUMCZ_BLOCKS, 256, 0, s>>>(mode, xb, p1, p2, nc, 0, sc + 1);
+  const int grid = launch_cap((int64_t)std::max(nsteps, 1) * TLINES, 256, 1184);
+  if (nv == 1)
+    k_quantT<1><<<grid, 256, 0, s>>>(mode, x, nullptr, p1, p2, nc, nsteps * TLINES, sc, dig1, dig2, v->d_col, qna_full,
+                                     na_second);
+  else
+    k_quantT<2><<<grid, 256, 0, s>>>(mode, x, xb, p1, p2, nc, nsteps * TLINES, sc, dig1, dig2, nullptr, nullptr, 0);
+  count_launch(xb ? 3 : 2);
   return BSG_OK;
 }
 
@@ -1806,7 +1651,7 @@ static int prodvec_T(bsg_view *v, const double *x_dev, double *out_dev, cudaStre
     qna = v->s_q1.as<long long>();
     BSG_CUDA(cudaMemsetAsync(qna, 0, (size_t)h->m * sizeof(long long), s));
   }
-  BSG_TRY(prep_T(v, mode, x_dev, v->d_center, v->d_scale, two, s, qna, v->has_scaling ? 1 : 0));  // incl. the partials of C
+  BSG_TRY(prep_T(v, mode, x_dev, v->d_center, v->d_scale, 1, nullptr, two, s, qna, v->has_scaling ? 1 : 0));
   long long *part = nullptr;
   BSG_TRY(run_pmvT(v, v->s_dig1.as<uint8_t>(), (h->has_na && !lists) ? 1 : 0,
                    two ? v->s_dig2.as<uint8_t>() : v->s_dig1.as<uint8_t>(), &part, s));
@@ -1819,7 +1664,7 @@ static int prodvec_T(bsg_view *v, const double *x_dev, double *out_dev, cudaStre
   if (comm && v->row_identity)  // epilogue fused with the sum over the column shards (NVLink peer memory, bsg_comm.cu)
     return comm_finish_prod_allreduce(comm, part, n, sc, v->has_scaling, h->has_na, out_dev, s);
   if (n > 0) {
-    k_finish_prod<<<(n + 255) / 256, 256, 0, s>>>(part, 1, n, n, sc, v->has_scaling, h->has_na, full);
+    k_finish_prod<<<(n + 255) / 256, 256, 0, s>>>(part, n, sc, v->has_scaling, h->has_na, full);
     count_launch();
   }
   if (!v->row_identity && v->nr > 0) {
@@ -1831,33 +1676,17 @@ static int prodvec_T(bsg_view *v, const double *x_dev, double *out_dev, cudaStre
   return BSG_OK;
 }
 
-// X~ [xa | xb] from the SNP-major copy in ONE pass over the matrix (two vectors, 4 + 4 digit slices; see k_quantT_pair).
+// X~ [xa | xb] from the SNP-major copy in ONE pass over the matrix (two vectors, 4 + 4 digit slices; see k_quantT).
 // xb / outb may be null (odd count).  Outputs in the caller's row order.
 static int prodvec_T_pair(bsg_view *v, const double *xa, const double *xb, double *outa, double *outb, cudaStream_t s) {
   using namespace pmv;
   using namespace pmvt;
   bsg_bed *h = v->h;
   Scal *sc = v->s_scal.as<Scal>();
-  const int n = h->n, nc = v->nc;
+  const int n = h->n;
   const int mode = v->has_scaling ? 1 : 0;
   const bool two = v->has_scaling && h->has_na;  // the NA plane has its own digits ((c - 3) z); else it reuses the raw ones
-  const int nsteps = (nc + TLINES - 1) / TLINES;
-  BSG_TRY(v->s_dig1.ensure((size_t)std::max(nsteps, 1) * 256));
-  if (two) BSG_TRY(v->s_dig2.ensure((size_t)std::max(nsteps, 1) * 256));
-  for (int vv = 0; vv < 2; vv++) {
-    const double *x = vv ? xb : xa;
-    k_scal_reset<<<1, 1, 0, s>>>(sc + vv);
-    count_launch();
-    if (!x) continue;
-    k_maxabs<<<launch_cap(nc, 256, 592), 256, 0, s>>>(mode, x, v->d_center, v->d_scale, nc, sc + vv);
-    if (v->has_scaling) k_sum_cz<<<SUMCZ_BLOCKS, 256, 0, s>>>(x, v->d_center, v->d_scale, nc, sc[vv].cpart);
-    count_launch(v->has_scaling ? 2 : 1);
-  }
-  k_pick_exp_pair<<<1, 32, 0, s>>>(sc, 0);
-  k_quantT_pair<<<launch_cap((int64_t)std::max(nsteps, 1) * TLINES, 256, 1184), 256, 0, s>>>(
-      mode, xa, xb, v->d_center, v->d_scale, nc, nsteps * TLINES, sc, v->s_dig1.as<uint8_t>(),
-      two ? v->s_dig2.as<uint8_t>() : nullptr);
-  count_launch(2);
+  BSG_TRY(prep_T(v, mode, xa, v->d_center, v->d_scale, 2, xb, two, s));
   long long *part = nullptr;
   BSG_TRY(run_pmvT(v, v->s_dig1.as<uint8_t>(), h->has_na ? 1 : 0, two ? v->s_dig2.as<uint8_t>() : v->s_dig1.as<uint8_t>(),
                    &part, s));
@@ -1903,41 +1732,12 @@ int bsg::view_prodvec_comm(bsg_view *v, const double *x_dev, double *out_dev, cu
   if (use_T(h)) return prodvec_T(v, x_dev, out_dev, s, comm);  // transposing kernel over the SNP-major copy
   using namespace pmv;
   Scal *sc = v->s_scal.as<Scal>();
-  const int m = h->m;
-  int nchunks = (int)(h->strideB / SEG);
   const int mode = v->has_scaling ? 1 : 0;
   const bool two = v->has_scaling && h->has_na;
-  BSG_TRY(v->s_q0.ensure((size_t)m * sizeof(long long)));
-  BSG_TRY(v->s_dig1.ensure((size_t)nchunks * DIG));
-  if (two) {
-    BSG_TRY(v->s_q1.ensure((size_t)m * sizeof(long long)));
-    BSG_TRY(v->s_dig2.ensure((size_t)nchunks * DIG));
-  }
-  long long *Q0 = v->s_q0.as<long long>();
-  long long *Q1 = two ? v->s_q1.as<long long>() : nullptr;
-  const int hb = hb_bits(v->col_maxmult);
-  if (v->col_identity) {
-    BSG_CUDA(cudaMemsetAsync(sc, 0, sizeof(Scal), s));
-    k_prep1<<<SUMCZ_BLOCKS, 256, 0, s>>>(mode, x_dev, v->d_center, v->d_scale, v->nc, hb, sc);
-    k_prep2<<<launch_cap((int64_t)nchunks * 32, 128, 1184), 128, 0, s>>>(
-        mode, x_dev, v->d_center, v->d_scale, m, nchunks, sc, v->s_dig1.as<uint8_t>(),
-        two ? v->s_dig2.as<uint8_t>() : nullptr, 0);
-    count_launch(2);
-  } else {
-    k_scal_reset<<<1, 1, 0, s>>>(sc);
-    k_maxabs<<<launch_cap(v->nc, 256, 592), 256, 0, s>>>(mode, x_dev, v->d_center, v->d_scale, v->nc, sc);
-    k_pick_exp<<<1, 1, 0, s>>>(sc, hb);
-    BSG_CUDA(cudaMemsetAsync(Q0, 0, (size_t)m * sizeof(long long), s));
-    if (Q1) BSG_CUDA(cudaMemsetAsync(Q1, 0, (size_t)m * sizeof(long long), s));
-    k_quantise<<<launch_cap(v->nc, 256, 592), 256, 0, s>>>(mode, x_dev, v->d_center, v->d_scale, v->nc, v->d_col, sc, Q0, Q1);
-    k_digits<<<launch_cap((int64_t)nchunks * 256, 256, 1184), 256, 0, s>>>(Q0, m, nchunks, v->s_dig1.as<uint8_t>());
-    if (Q1) k_digits<<<launch_cap((int64_t)nchunks * 256, 256, 1184), 256, 0, s>>>(Q1, m, nchunks, v->s_dig2.as<uint8_t>());
-    if (v->has_scaling) k_sum_cz<<<SUMCZ_BLOCKS, 256, 0, s>>>(x_dev, v->d_center, v->d_scale, v->nc, sc->cpart);
-    count_launch(5 + (Q1 ? 1 : 0) + (v->has_scaling ? 1 : 0));
-  }
+  BSG_TRY(prep_pmv(v, 0, mode, x_dev, v->d_center, v->d_scale, 1, nullptr, two, false, false, s));
   Args a;
   const int nlines = v->row_identity ? h->n : v->nru;
-  BSG_TRY(run_pmv(v, h->B, h->strideB, m, v->d_rows_unique, nlines, v->s_dig1.as<uint8_t>(),
+  BSG_TRY(run_pmv(v, h->B, h->strideB, h->m, v->d_rows_unique, nlines, v->s_dig1.as<uint8_t>(),
                   two ? v->s_dig2.as<uint8_t>() : nullptr, h->naB, h->has_na, &a, s));
   double *full = out_dev;
   if (!v->row_identity) {
@@ -1946,8 +1746,7 @@ int bsg::view_prodvec_comm(bsg_view *v, const double *x_dev, double *out_dev, cu
   }
   if (comm && v->row_identity)
     return comm_finish_prod_allreduce(comm, a.part, nlines, sc, v->has_scaling, h->has_na, out_dev, s);
-  k_finish_prod<<<(nlines + 255) / 256, 256, 0, s>>>(a.part, a.ksplit, a.nlines_pad, nlines, sc, v->has_scaling,
-                                                     h->has_na, full);
+  k_finish_prod<<<(nlines + 255) / 256, 256, 0, s>>>(a.part, nlines, sc, v->has_scaling, h->has_na, full);
   count_launch();
   if (!v->row_identity) {
     k_gather<<<(v->nr + 255) / 256, 256, 0, s>>>(full, v->d_row_gather, v->nr, out_dev);
@@ -2114,7 +1913,7 @@ static int view_planes_dev(bsg_view *v, int dir, const double *x1, const double 
   Scal *sc = v->s_scal.as<Scal>();
   if (dir == 0 && use_T(h)) {
     // X-side sums from the SNP-major copy: raw-plane launch + flag-plane launch of k_pmvT
-    BSG_TRY(prep_T(v, two ? 2 : 0, x1, x2, nullptr, two, s));
+    BSG_TRY(prep_T(v, two ? 2 : 0, x1, x2, nullptr, 1, nullptr, two, s));
     long long *part = nullptr;
     BSG_TRY(run_pmvT(v, v->s_dig1.as<uint8_t>(), plane == PLANE_NONE ? 0 : (plane == PLANE_NA ? 1 : 2),
                      two ? v->s_dig2.as<uint8_t>() : v->s_dig1.as<uint8_t>(), &part, s));
@@ -2137,39 +1936,10 @@ static int view_planes_dev(bsg_view *v, int dir, const double *x1, const double 
     BSG_CUDA(cudaGetLastError());
     return BSG_OK;
   }
-  const int L = dir == 0 ? h->m : h->n;                      // contraction length in the staged copy
-  const int len = dir == 0 ? v->nc : v->nr;                  // vector length (selection order)
-  const int *idx = dir == 0 ? v->d_col : v->d_row;
-  const bool ident = dir == 0 ? v->col_identity : v->row_identity;
-  const int hb = hb_bits(dir == 0 ? v->col_maxmult : v->row_maxmult);
+  BSG_TRY(prep_pmv(v, dir, two ? 2 : 0, x1, x2, nullptr, 1, nullptr, two, false, false, s));
+  const int L = dir == 0 ? h->m : h->n;  // contraction length in the staged copy
   const int64_t stride = dir == 0 ? h->strideB : h->strideA;
-  const int nchunks = (int)(stride / SEG);
-  const int mode = two ? 2 : 0;
-  BSG_TRY(v->s_dig1.ensure((size_t)nchunks * DIG));
-  if (two) BSG_TRY(v->s_dig2.ensure((size_t)nchunks * DIG));
   uint8_t *dig1 = v->s_dig1.as<uint8_t>(), *dig2 = two ? v->s_dig2.as<uint8_t>() : nullptr;
-  if (ident) {
-    BSG_CUDA(cudaMemsetAsync(sc, 0, sizeof(Scal), s));
-    k_prep1<<<SUMCZ_BLOCKS, 256, 0, s>>>(mode, x1, x2, nullptr, len, hb, sc);
-    k_prep2<<<launch_cap((int64_t)nchunks * 32, 128, 1184), 128, 0, s>>>(mode, x1, x2, nullptr, L, nchunks, sc, dig1, dig2, 0);
-    count_launch(2);
-  } else {
-    BSG_TRY(v->s_q0.ensure((size_t)L * sizeof(long long)));
-    long long *Q0 = v->s_q0.as<long long>(), *Q1 = nullptr;
-    if (two) {
-      BSG_TRY(v->s_q1.ensure((size_t)L * sizeof(long long)));
-      Q1 = v->s_q1.as<long long>();
-    }
-    k_scal_reset<<<1, 1, 0, s>>>(sc);
-    k_maxabs<<<launch_cap(len, 256, 592), 256, 0, s>>>(mode, x1, x2, nullptr, len, sc);
-    k_pick_exp<<<1, 1, 0, s>>>(sc, hb);
-    BSG_CUDA(cudaMemsetAsync(Q0, 0, (size_t)L * sizeof(long long), s));
-    if (Q1) BSG_CUDA(cudaMemsetAsync(Q1, 0, (size_t)L * sizeof(long long), s));
-    k_quantise<<<launch_cap(len, 256, 592), 256, 0, s>>>(mode, x1, x2, nullptr, len, idx, sc, Q0, Q1);
-    k_digits<<<launch_cap((int64_t)nchunks * 256, 256, 1184), 256, 0, s>>>(Q0, L, nchunks, dig1);
-    if (Q1) k_digits<<<launch_cap((int64_t)nchunks * 256, 256, 1184), 256, 0, s>>>(Q1, L, nchunks, dig2);
-    count_launch(5 + (Q1 ? 1 : 0));
-  }
   Args a;
   int nlines;
   if (dir == 0) {
@@ -2201,7 +1971,7 @@ static int view_planes_dev(bsg_view *v, int dir, const double *x1, const double 
 }
 
 
-// Xt-side plane sums of TWO vectors in one pass over the SNP-major copy (30-bit fixed point each, see k_pick_exp_pair):
+// Xt-side plane sums of TWO vectors in one pass over the SNP-major copy (30-bit fixed point each, see pick_e):
 // per vector R_l = sum_t code(l, t) x[t] and, with plane == PLANE_NA, N_l = sum_t [missing(l, t)] x[t].
 static int view_planes_pair_dev(bsg_view *v, const double *xa, const double *xb, int plane, const pmvt::PairCoef &ca,
                                 const pmvt::PairCoef &cb, cudaStream_t s) {
@@ -2209,33 +1979,11 @@ static int view_planes_pair_dev(bsg_view *v, const double *xa, const double *xb,
   bsg_bed *h = v->h;
   if (plane == PLANE_NA && !h->has_na) plane = PLANE_NONE;
   Scal *sc = v->s_scal.as<Scal>();
-  const int L = h->n, len = v->nr;
-  const int hb = hb_bits(v->row_maxmult);
-  const int64_t stride = h->strideA;
-  const int nchunks = (int)(stride / SEG);
-  BSG_TRY(v->s_dig1.ensure((size_t)nchunks * DIG));
-  BSG_TRY(v->s_q0.ensure((size_t)L * sizeof(long long)));
-  BSG_TRY(v->s_q1.ensure((size_t)L * sizeof(long long)));
-  uint8_t *dig1 = v->s_dig1.as<uint8_t>();
-  long long *Q0 = v->s_q0.as<long long>(), *Q1 = v->s_q1.as<long long>();
-  const int *idx = v->row_identity ? nullptr : v->d_row;
-  k_scal_reset<<<1, 1, 0, s>>>(sc);
-  k_scal_reset<<<1, 1, 0, s>>>(sc + 1);
-  k_maxabs<<<launch_cap(len, 256, 592), 256, 0, s>>>(0, xa, nullptr, nullptr, len, sc);
-  if (xb) k_maxabs<<<launch_cap(len, 256, 592), 256, 0, s>>>(0, xb, nullptr, nullptr, len, sc + 1);
-  pmvt::k_pick_exp_pair<<<1, 32, 0, s>>>(sc, hb);
-  if (idx) {
-    BSG_CUDA(cudaMemsetAsync(Q0, 0, (size_t)L * sizeof(long long), s));
-    BSG_CUDA(cudaMemsetAsync(Q1, 0, (size_t)L * sizeof(long long), s));
-  }
-  k_quantise<<<launch_cap(len, 256, 592), 256, 0, s>>>(0, xa, nullptr, nullptr, len, idx, sc, Q0, nullptr);
-  if (xb) k_quantise<<<launch_cap(len, 256, 592), 256, 0, s>>>(0, xb, nullptr, nullptr, len, idx, sc + 1, Q1, nullptr);
-  pmvt::k_digits_pair<<<launch_cap((int64_t)nchunks * 256, 256, 1184), 256, 0, s>>>(Q0, xb ? Q1 : nullptr, idx ? L : len, nchunks,
-                                                                                  dig1);
-  count_launch(6 + (xb ? 2 : 0));
+  BSG_TRY(prep_pmv(v, 1, 0, xa, nullptr, nullptr, 2, xb, false, false, false, s));
   Args a;
   const int nlines = v->nc;
-  BSG_TRY(run_pmv(v, h->A, stride, L, v->d_col, nlines, dig1, nullptr, h->naA, plane != PLANE_NONE, &a, s, false));
+  BSG_TRY(run_pmv(v, h->A, h->strideA, h->n, v->d_col, nlines, v->s_dig1.as<uint8_t>(), nullptr, h->naA,
+                  plane != PLANE_NONE, &a, s, false));
   pmvt::k_finish_planes_pair<<<(nlines + 255) / 256, 256, 0, s>>>(a.part, nlines, sc, plane != PLANE_NONE, ca, cb);
   count_launch();
   BSG_CUDA(cudaGetLastError());
@@ -2415,7 +2163,7 @@ int bsg_prod_and_rowsumssq(bsg_bed *h, const int *ind_row, int nr, const int *in
     pair_mode = (ev && ev[0] == '0') ? 0 : 1;
   }
   if (pair_mode && K >= 2) {
-    // two columns of V per pass over the matrix (30-bit fixed point per vector, see k_quantT_pair)
+    // two columns of V per pass over the matrix (30-bit fixed point per vector, see k_quantT)
     for (int k = 0; k < K; k += 2) {
       const bool both = k + 1 < K;
       BSG_TRY(upload(k, std::min(K, k + 2)));

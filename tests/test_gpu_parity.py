@@ -190,7 +190,7 @@ def test_single_copy_kernel_matches_oracle(B, oracle, obed, obed_na, rng):
         V = rng.normal(size=(M, 3))
         XV, rss = B.prod_and_rowSumsSq(g1, ir, ic, sc["center"], sc["scale"], V)
         XVo, rsso = oracle.prod_and_rowSumsSq(o, ir, ic, sc["center"], sc["scale"], V)
-        _close(XV, XVo, tol=1e-8)  # two columns of V per pass: 30-bit fixed point per vector (bsg_pmv.cu k_quantT_pair)
+        _close(XV, XVo, tol=1e-8)  # two columns of V per pass: 30-bit fixed point per vector (bsg_pmv.cu k_quantT<2>)
         _close(rss, rsso, tol=1e-12)
         y = rng.normal(size=M)
         y[5] = np.nan
@@ -469,7 +469,7 @@ def test_prod_and_rowSumsSq_and_projection(B, gbed, gbed_na, oracle, obed, obed_
             V = rng.normal(size=(ic.size, 4))
             XV, rss = B.prod_and_rowSumsSq(g, ir, ic, c, s, V)
             XVo, rsso = oracle.prod_and_rowSumsSq(o, ir, ic, c, s, V)
-            _close(XV, XVo, tol=1e-8)  # two columns of V per pass: 30-bit fixed point per vector (bsg_pmv.cu k_quantT_pair)
+            _close(XV, XVo, tol=1e-8)  # two columns of V per pass: 30-bit fixed point per vector (bsg_pmv.cu k_quantT<2>)
             _close(rss, rsso, tol=1e-12)
         # identity scaling and a vector V
         ic = np.arange(1, m + 1)
@@ -483,7 +483,7 @@ def test_prod_and_rowSumsSq_and_projection(B, gbed, gbed_na, oracle, obed, obed_
     V = rng.normal(size=(ic.size, 2))
     XV, rss = B.prod_and_rowSumsSq(g1, ir, ic, sc["center"], sc["scale"], V)
     XVo, rsso = oracle.prod_and_rowSumsSq(obed_na, ir, ic, sc["center"], sc["scale"], V)
-    _close(XV, XVo, tol=1e-8)  # two columns of V per pass: 30-bit fixed point per vector (bsg_pmv.cu k_quantT_pair)
+    _close(XV, XVo, tol=1e-8)  # two columns of V per pass: 30-bit fixed point per vector (bsg_pmv.cu k_quantT<2>)
     _close(rss, rsso, tol=1e-12)
     # zero scale: the reference's Inf / NaN pattern (table arithmetic), not a crash
     s0 = sc["scale"].copy(); s0[3] = 0.0

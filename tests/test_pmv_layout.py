@@ -1,5 +1,5 @@
-"""Lane-level NumPy model of the tensor-pipe matvec kernel (bigsnpr_b200/csrc/bsg_pmv.cu: k_digits, tile_stage,
-k_pmv epilogue, combine8).  It replays the exact index arithmetic of the CUDA code -- digit layout in shared
+"""Lane-level NumPy model of the tensor-pipe matvec kernel (bigsnpr_b200/csrc/bsg_pmv.cu: k_prep2 digit layout,
+k_pmv fragments and epilogue, combine).  It replays the exact index arithmetic of the CUDA code -- digit layout in shared
 memory, mask decode of the packed words, mma.sync.m16n8k32 fragment ownership (PTX ISA: A row = groupID(+8),
 col = 4*tid_in_group + i (+16); B row = 4*tid_in_group + i (+16), col = groupID; C row = groupID(+8),
 col = 2*tid_in_group + i) -- and checks the result against exact integer dot products.  Runs on CPU: it
@@ -11,7 +11,7 @@ CODES, DIG = 512, 4096
 
 
 def digits_of(Q):
-    """signed base-256 digits, as k_digits peels them"""
+    """signed base-256 digits, as peel() takes them off"""
     out = []
     v = int(Q)
     for _ in range(8):
@@ -23,7 +23,7 @@ def digits_of(Q):
 
 
 def make_digit_chunk(Qchunk):
-    """k_digits: unit (w, s, q) at ((w*8+s)*4+q)*16, byte c*4+r <-> code
+    """k_prep2: unit (w, s, q) at ((w*8+s)*4+q)*16, byte c*4+r <-> code
     t = (64q + 16w if w < 4 else 256 + 64q + 16(w-4)) + 4r + c  (word w of lane q, see k_pmv slot_load)."""
     buf = np.zeros(DIG, dtype=np.int8)
     D = np.array([digits_of(q) for q in Qchunk], dtype=np.int64)  # (512, 8)
@@ -124,7 +124,7 @@ def test_pmv_layout_exact():
 
 
 def test_combine8_is_fp64_exact_enough():
-    """combine8: top-down fp64 sum of slice sums == exact integer / 2^e to 1 ulp."""
+    """combine<8>: top-down fp64 sum of slice sums == exact integer / 2^e to 1 ulp."""
     rng = np.random.default_rng(6)
     for _ in range(50):
         v = [int(x) for x in rng.integers(-(1 << 33), 1 << 33, size=8)]

@@ -38,9 +38,9 @@ def test_prmt_transpose_is_a_byte_transpose():
 
 
 def stage_strip(lines64, width):
-    """cp.async destinations of one warp stage.  lines64: (32, width) bytes (width = 64 for k_pmvT, 32 for k_pmvT2).
-    k_pmvT : word (row = 16 hf + 4 qq + r, column wc = 8 sl + gg) at word ((((r 2 + hf) 2 + sl) 4 + qq) 8 + gg)
-    k_pmvT2: word (row, column gg)                                 at word  (((r 2 + hf) 4 + qq) 8 + gg)"""
+    """cp.async destinations of one warp stage.  lines64: (32, width) bytes (width = 64 for k_pmvT_lines, 32 for k_pmvT2).
+    k_pmvT_lines: word (row = 16 hf + 4 qq + r, column wc = 8 sl + gg) at word ((((r 2 + hf) 2 + sl) 4 + qq) 8 + gg)
+    k_pmvT2:      word (row, column gg)                                 at word  (((r 2 + hf) 4 + qq) 8 + gg)"""
     smem = np.zeros(32 * width // 4, dtype=np.uint32)
     words = lines64.reshape(32, width // 4, 4)
     for lane in range(32):  # loader role: 4 (or 2) granules of 16 B per lane
