@@ -28,6 +28,8 @@ SIGNATURES = {
     "bsg_open_synth_ld": (C.c_int, [C.c_int, C.c_int, C.c_uint64, C.c_double, C.c_int64, C.c_double, C.c_int, C.c_int, C.c_int,
                                     C.POINTER(vp)]),
     "bsg_open_fbm256": (C.c_int, [c_u8_p, C.c_int, C.c_int, c_dbl_p, C.c_int, C.c_int, C.POINTER(vp)]),
+    "bsg_code256_dosage_scale": (C.c_int, [c_dbl_p]),
+    "bsg_dosage_scale": (C.c_int, [vp]),
     "bsg_close": (None, [vp]),
     "bsg_nrow": (C.c_int, [vp]),
     "bsg_ncol": (C.c_int, [vp]),
@@ -63,6 +65,8 @@ SIGNATURES = {
     "bsg_set_scaling_reuse": (C.c_int, [C.c_int]),
     "bsg_prod_and_rowsumssq": (C.c_int, [vp, c_int_p, C.c_int, c_int_p, C.c_int, c_dbl_p, c_dbl_p, c_dbl_p, C.c_int,
                                          c_dbl_p, c_dbl_p]),
+    "bsg_prod_and_rowsumssq2": (C.c_int, [vp, c_int_p, C.c_int, c_int_p, C.c_int, c_dbl_p, c_dbl_p, c_dbl_p, C.c_int,
+                                          c_dbl_p, c_dbl_p]),
     "bsg_multlinreg": (C.c_int, [vp, c_int_p, C.c_int, c_int_p, C.c_int, c_dbl_p, C.c_int, c_dbl_p]),
     "bsg_tcrossprod": (C.c_int, [vp, c_int_p, C.c_int, c_int_p, C.c_int, c_dbl_p, c_dbl_p, c_dbl_p]),
     "bsg_tcrossprod_dev": (C.c_int, [vp, c_int_p, C.c_int, c_int_p, C.c_int, c_dbl_p, c_dbl_p, vp]),

@@ -178,6 +178,12 @@ class Bed:
         return bool(lib().bsg_has_na(self._h))
 
     @property
+    def dosage_scale(self):
+        """D when this handle holds dosages whose finite codes are multiples of 1 / D in 0..255 / D (CODE_DOSAGE: 100):
+        such handles also serve bed_prodVec / bed_cprodVec and bed_randomSVD with an explicit fun_scaling.  0 otherwise."""
+        return int(lib().bsg_dosage_scale(self._h))
+
+    @property
     def layouts(self):
         return int(lib().bsg_layouts(self._h))
 
@@ -491,6 +497,15 @@ def snp_colstats(G, ind_row=..., ind_col=..., ncores=1):
     return {"sumX": sumX, "denoX": denoX}
 
 
+def code256_dosage_scale(code256):
+    """The smallest integer D in 1..255 such that D * v is an integer in 0..255 for every finite value v of the FBM.code256
+    table (and every other value is NA), else 0 (see include/bsgpu.h)."""
+    code256 = _f64(code256)
+    if code256.size != 256:
+        raise ValueError("code256 must have 256 values.")
+    return int(lib().bsg_code256_dosage_scale(_pd(code256)))
+
+
 def snp_scaleBinom(nploidy=2):
     """R/binom-scaling.R:62-77: returns the scaling function."""
 
@@ -732,8 +747,13 @@ def _auto_svd(obj_bed, infos_chr, infos_pos, ind_row, ind_col, fun_scaling, thr_
     say = print if verbose else (lambda *a, **k: None)
     if not (min_mac > 0 and min_maf > 0):
         raise ValueError("You cannot use variants with no variation; set min.mac > 0 and min.maf > 0.")
-    info = bed_MAF(obj_bed, ind_row, ind_col, ncores)
-    nok = (info["mac"] < min_mac) | (info["maf"] < min_maf)
+    if fbm and obj_bed.dosage_scale:
+        # dosages have no hard-call counts: R/autoSVD.R:96-101, snp_MAF and maf < max(min.maf, min.mac / (2 n))
+        maf = snp_MAF(obj_bed, ind_row, ind_col, ncores=ncores)
+        nok = maf < max(min_maf, min_mac / (2 * ind_row.size))
+    else:
+        info = bed_MAF(obj_bed, ind_row, ind_col, ncores)
+        nok = (info["mac"] < min_mac) | (info["maf"] < min_maf)
     say("Discarding %d variant%s with MAC < %s or MAF < %s." % (nok.sum(), "s" if nok.sum() > 1 else "", min_mac, min_maf))
     ind_keep = ind_col[~nok]
     if thr_r2 is None or np.isnan(thr_r2):
@@ -842,6 +862,39 @@ def prod_and_rowSumsSq(obj_bed, ind_row, ind_col, center, scale, V):
                                        _pd(scale), V.ctypes.data_as(_lib.c_dbl_p), K,
                                        XV.ctypes.data_as(_lib.c_dbl_p), _pd(rss)))
     return XV, rss
+
+
+def prod_and_rowSumsSq2(G, ind_row, ind_col, center, scale, V):
+    """src/project-utils.cpp:11-43 on an FBM.code256 handle -> (XV (nr, K), rowSumsSq (nr)); an NA code is NA_real, so a
+    row holding one in a selected column is NaN in both outputs."""
+    ind_row, ind_col = _i32(ind_row), _i32(ind_col)
+    center, scale = _f64(center), _f64(scale)
+    V = np.asarray(V, dtype=np.float64)
+    V = np.asfortranarray(V.reshape(V.shape[0], -1))
+    if center.size != ind_col.size or scale.size != ind_col.size or V.shape[0] != ind_col.size:
+        raise ValueError(ERROR_DIM)
+    K = V.shape[1]
+    XV = np.empty((ind_row.size, K), dtype=np.float64, order="F")
+    rss = np.empty(ind_row.size, dtype=np.float64)
+    check(lib().bsg_prod_and_rowsumssq2(G._h, _pi(ind_row), ind_row.size, _pi(ind_col), ind_col.size, _pd(center),
+                                        _pd(scale), V.ctypes.data_as(_lib.c_dbl_p), K,
+                                        XV.ctypes.data_as(_lib.c_dbl_p), _pd(rss)))
+    return XV, rss
+
+
+def snp_projectSelfPCA(obj_svd, G, ind_row, ind_col=None, ncores=1):
+    """R/bed-projectPCA.R:252-281: project the samples `ind_row` of the FBM.code256 `G` on the PCs of `obj_svd` (dict with
+    v, d, center, scale; `ind_col` defaults to its "subset").  Returns obj.svd.ref, simple_proj (= XV) and X_norm (row sums
+    of squares); the OADP correction is bigutilsr::pca_OADP_proj2 on the host (un-vendored R code), as bed_projectSelfPCA."""
+    v = np.asarray(obj_svd["v"], dtype=np.float64)
+    if ind_col is None:
+        ind_col = obj_svd.get("subset", None)
+    if ind_col is None:
+        raise ValueError("'ind.col' can't be `NULL`.")
+    ind_row, ind_col = _i32(ind_row), _i32(ind_col)
+    _assert_lengths(np.arange(v.shape[0]), ind_col)
+    XV, x_norm = prod_and_rowSumsSq2(G, ind_row, ind_col, obj_svd["center"], obj_svd["scale"], v)
+    return {"obj.svd.ref": obj_svd, "simple_proj": XV, "X_norm": x_norm}
 
 
 def bed_projectSelfPCA(obj_svd, obj_bed, ind_row, ind_col=None, ncores=1):

@@ -678,6 +678,7 @@ int bsg_open_fbm256(const uint8_t *bytes, int n, int m, const double *code256, i
   }
   if (generic && !rc) {  // keep the code bytes and the table: bsg_generic.cu reads code256[byte] like SubBMCode256Acc does
     h->fbm_generic = 1;
+    h->dos_scale = dosage_scale_of(code256);
     h->raw = draw;
     draw = nullptr;
     double both[512];
@@ -708,8 +709,9 @@ void bsg_close(bsg_bed *h) {
     bsg_view_destroy(h->cv);
     h->cv = nullptr;
   }
-  void *ptrs[] = {h->A, h->B, h->cntA, h->cntB, h->naA, h->naB, h->raw, h->d_code, h->ellCnt[0], h->ellCnt[1], h->ellEnt[0],
-                  h->ellEnt[1], h->ellOff[0], h->ellOff[1], h->ellOut[0], h->ellOut[1]};
+  void *ptrs[] = {h->A, h->B, h->cntA, h->cntB, h->naA, h->naB, h->raw, h->d_code, h->dosV, h->dosNaCnt, h->dosNa,
+                  h->ellCnt[0], h->ellCnt[1], h->ellEnt[0], h->ellEnt[1], h->ellOff[0], h->ellOff[1], h->ellOut[0],
+                  h->ellOut[1]};
   for (void *p : ptrs)
     if (p) cudaFree(p);
   DevBuf *bufs[] = {&h->w_idx_row, &h->w_idx_col, &h->w_center, &h->w_scale, &h->w_x, &h->w_out, &h->w_tmp0,

@@ -98,6 +98,17 @@ struct bsg_bed {
   int fbm_generic = 0;       // FBM whose codes are not {0,1,2,NA} (dosages ...): served by the fp64 kernels of bsg_generic.cu
   uint8_t *raw = nullptr;    // generic FBM: the n x m code bytes, column-major, as in the .bk file
   double *d_code = nullptr;  // generic FBM: code256 on the device [0,256) and the same with NA -> 3 [256,512)
+  // dosage FBM (generic, every finite code a multiple of 1 / dos_scale: bsg_code256_dosage_scale): the byte-operand
+  // products of bsg_dosage.cu read a value copy built on first use.  dosV: m lines of dosStride = round_up(n, 128) bytes,
+  // byte = round(dos_scale * code256[raw]) in 0..255, NA codes and pads 0 (+ 512 bytes of slack for the last line's
+  // segment loads); dosNaCnt[m]: NA codes per line; dosNa: the dosNaTotal (line, sample) positions of NA codes, in line
+  // order, used only to set the outputs they touch to NaN.
+  int dos_scale = 0;
+  uint8_t *dosV = nullptr;
+  int64_t dosStride = 0;
+  int32_t *dosNaCnt = nullptr;
+  int2 *dosNa = nullptr;
+  int64_t dosNaTotal = 0;
   cudaStream_t stream = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   cudaStream_t copy_stream = nullptr;  // created on first use: host -> device uploads that run under the kernels of `stream`
@@ -183,6 +194,7 @@ int generic_colstats(bsg_bed *h, const int *d_row, int nr, const int *d_col, int
 int generic_pairs(bsg_bed *h, const int *d_row, int nr, const int *d_col, int nc, int kind, const int *d_wlen,
                   const long long *d_boff, long long total, const double *d_thr, double *d_band, uint8_t *d_keep,
                   const double *d_sumX, const double *d_denoX, double thr_r2, cudaStream_t s);
+int dosage_scale_of(const double *code256);  // the D of bsg_code256_dosage_scale (0: not a dosage table)
 int generic_multlinreg(bsg_bed *h, const int *d_row, int nr, const int *d_col, int nc, const double *d_U, int K,
                        double *d_out, cudaStream_t s);
 
@@ -201,6 +213,20 @@ struct PmvPlan;  // opaque, owned by a view
 namespace pmv { struct Scal; }
 // X~ x enqueued on `s`; with a communicator the partial n-vectors of the column shards are summed (fused epilogue)
 int view_prodvec_comm(bsg_view *v, const double *x_dev, double *out_dev, cudaStream_t s, bsg_comm *comm);
+
+// ---- bsg_dosage.cu: X.y / Xt.y of dosage FBM handles on the integer tensor pipe, from the value copy ----------------
+int dosage_build(bsg_bed *h);           // value copy + NA list (no-op when resident)
+int dosage_view_masks(bsg_view *v);     // selected-row / selected-column flags (only when the matrix has NA codes)
+int dosage_prodvec(bsg_view *v, const double *x_dev, double *out_dev, cudaStream_t s);
+int dosage_cprodvec(bsg_view *v, const double *x_dev, double *out_dev, cudaStream_t s);
+int dosage_literal(bsg_view *v, bool cprod, const double *x_dev, double *out_dev, cudaStream_t s);  // per-element fp64
+// prod_and_rowSumsSq2 of an FBM handle (dosage or hard calls) as the reference's loop: rss, per-row NA flag and, for K > 0,
+// XV += (pre-zeroed); then XV rows holding an NA code set to NaN
+int fbm_proj_literal(bsg_view *v, const double *d_V, int K, double *d_XV, double *d_rss, uint8_t *d_na, cudaStream_t s);
+int fbm_nan_rows(const uint8_t *d_na, int nr, int K, double *d_XV, cudaStream_t s);
+// bsg_pmv.cu: the vector preparation these kernels share with the 2-bit ones
+int dosage_prep_cols(bsg_view *v, const double *x_dev, cudaStream_t s);
+int dosage_prep_rows(bsg_view *v, const double *x_dev, long long *Q, cudaStream_t s);
 
 // ---- bsg_la.cu: the Lanczos driver over one or several column shards (one replica of the recurrence per shard) ----
 struct SvdShard {
@@ -241,4 +267,6 @@ struct bsg_view {
   int nru = 0;
   // scratch owned by the view (so device-pointer calls are allocation free)
   bsg::DevBuf s_vec0, s_vec1, s_q0, s_q1, s_dig1, s_dig2, s_part, s_scal, s_full;
+  // dosage handles with NA codes: 1 per selected sample [n] / SNP column [m] (null if identity or no NA code)
+  uint8_t *d_rowsel = nullptr, *d_colsel = nullptr;
 };

@@ -73,54 +73,6 @@ struct Args {
   long long *part;       // [nlines_pad][16] zeroed accumulators: 8 raw-plane slices, 8 NA-plane slices
 };
 
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "WAIT_%=:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-      "@p bra DONE_%=;\n\t"
-      "bra WAIT_%=;\n\t"
-      "DONE_%=:\n\t}" ::"r"(bar),
-      "r"(parity)
-      : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void *src, uint32_t bytes, uint32_t bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
-               "l"(src), "r"(bytes), "r"(bar)
-               : "memory");
-}
-__device__ __forceinline__ void mma_u8s8(int (&d)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3,
-                                         uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k32.row.col.s32.u8.s8.s32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3])
-      : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ uint4 lds128(uint32_t addr) {
-  uint4 v;
-  asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr));
-  return v;
-}
-
-__device__ __forceinline__ uint4 ldg_stream(const uint8_t *p) {
-  uint4 v;
-  asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];"
-               : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w)
-               : "l"(p));
-  return v;
-}
-
 // Fragment bytes of one lane for one 16-line sub-tile and one 128-byte chunk: lines g (a*) and g+8 (b*),
 // bytes [16q, 16q+16) (lo) and [64+16q, 64+16q+16) (hi) of the chunk.
 struct Slot {
@@ -387,24 +339,6 @@ __device__ __forceinline__ void make_vals(int mode, const double *x, const doubl
   }
 }
 
-// e = bits - exponent(maxabs) - hb, so that |sum of <= 2^hb quantised values| < 2^bits.  bits = 60: one vector in 8
-// signed base-256 digits; bits = 30: one of two vectors sharing a pass in 4 digits (max 127 * (2^32 - 1) / 255).
-__device__ __forceinline__ int pick_e(double m, int hb, int bits) {
-  int ex = 0;
-  if (m > 0 && isfinite(m)) {
-    frexp(m, &ex);
-    return bits - ex - hb;
-  }
-  return 0;
-}
-
-// the next signed base-256 digit of q (its low byte as int8); q keeps the exact rest (q - d) / 256
-__device__ __forceinline__ int peel(long long &q) {
-  const int d = (int)(signed char)(q & 0xFF);
-  q = (q - d) >> 8;
-  return d;
-}
-
 // pass 1 on every path: max |v0|, max |v1|, finiteness and, for X.y with scaling, the per-block partials of
 // C = sum_k c_k z_k.  Fixed grid of SUMCZ_BLOCKS blocks; one launch per vector.
 __global__ void k_prep1(int mode, const double *__restrict__ x, const double *__restrict__ center,
@@ -443,7 +377,7 @@ __global__ void k_prep1(int mode, const double *__restrict__ x, const double *__
   }
 }
 
-// Scatter of an index multiset (`ind.row` / `ind.col`): Q[idx[k]] += rint(v * 2^e) into a pre-zeroed Q, so duplicates
+// Scatter of an index multiset (`ind.row` / `ind.col`; idx == null: the identity): Q[idx[k]] += rint(v * 2^e) into a pre-zeroed Q, so duplicates
 // add up in integers (order independent).  The exponents follow from what k_prep1 left in *sc.
 __global__ void k_quantise(int mode, const double *__restrict__ x, const double *__restrict__ center,
                            const double *__restrict__ scale, int len, const int *__restrict__ idx, const Scal *sc, int bits,
@@ -454,10 +388,11 @@ __global__ void k_quantise(int mode, const double *__restrict__ x, const double 
     double v0, v1;
     make_vals(mode, x, center, scale, k, v0, v1);
     const long long q0 = bad ? 0 : __double2ll_rn(scalbn(v0, e0));
-    atomicAdd(reinterpret_cast<unsigned long long *>(Q0 + idx[k]), (unsigned long long)q0);
+    const int t = idx ? idx[k] : k;
+    atomicAdd(reinterpret_cast<unsigned long long *>(Q0 + t), (unsigned long long)q0);
     if (Q1) {
       const long long q1 = bad ? 0 : __double2ll_rn(scalbn(v1, e1));
-      atomicAdd(reinterpret_cast<unsigned long long *>(Q1 + idx[k]), (unsigned long long)q1);
+      atomicAdd(reinterpret_cast<unsigned long long *>(Q1 + t), (unsigned long long)q1);
     }
   }
 }
@@ -794,16 +729,6 @@ struct TArgs {
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void *src, int src_bytes) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
 }
-__device__ __forceinline__ uint32_t lds32(uint32_t addr) {
-  uint32_t v;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(addr));
-  return v;
-}
-__device__ __forceinline__ uint32_t prmt(uint32_t a, uint32_t b, uint32_t sel) {
-  uint32_t r;
-  asm("prmt.b32 %0, %1, %2, %3;" : "=r"(r) : "r"(a), "r"(b), "r"(sel));
-  return r;
-}
 
 // Line list (a.lines): per-warp cp.async strips.
 template <int PLANE>
@@ -955,15 +880,6 @@ constexpr int TSTAGE_BYTES = 4 * TBOX + 1024;                // + digits; stages
 constexpr int TCSTAGES = 6;                                  // 100 KB of stages per CTA, 2 CTAs per SM
 constexpr int TSMEM_TMA = TCSTAGES * TSTAGE_BYTES + 2 * TCSTAGES * 8 + 1024;  // + mbarriers + alignment slack
 
-__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap *map, uint32_t bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(dst),
-      "l"(map), "r"(bar), "r"(c0), "r"(c1)
-      : "memory");
-}
-
-// address bits of read i (row i, chunk ^ i) and of word column half sl (chunk ^ 2 sl), relative to the lane's i = sl = 0
-__host__ __device__ constexpr uint32_t TRD(int i, int sl) { return (uint32_t)((i << 7) ^ (i << 4) ^ (sl << 5)); }
 
 template <int PLANE>
 __global__ void __launch_bounds__(TWARPS * 32, 2) k_pmvT(const __grid_constant__ CUtensorMap map, const TArgs a) {
@@ -1385,8 +1301,10 @@ int bsg_view_create(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, 
                     const double *scale, bsg_view **out) {
   if (!h || !out) return fail(BSG_ERR_ARG, "null argument");
   *out = nullptr;
-  BSG_PACKED_ONLY(h, "The packed matrix-vector engine");
+  // dosage FBM handles whose codes are multiples of 1 / D (bsg_code256_dosage_scale) run on their value copy
+  if (!h->dos_scale) BSG_PACKED_ONLY(h, "The packed matrix-vector engine");
   BSG_TRY(bind_device(h));
+  if (h->fbm_generic) BSG_TRY(dosage_build(h));
   if (!ind_row) nr = h->n;
   if (!ind_col) nc = h->m;
   if (nr < 0 || nc < 0) return fail(BSG_ERR_ARG, "negative length");
@@ -1447,6 +1365,7 @@ int bsg_view_create(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, 
     if (!rc) rc = dev_copy((void **)&v->d_scale, scale, (size_t)nc * sizeof(double), s);
   }
   if (!rc) rc = v->s_scal.ensure(2 * sizeof(pmv::Scal));  // the second block serves the two-vectors-per-pass mode
+  if (!rc && h->fbm_generic) rc = dosage_view_masks(v);
   cudaError_t e = cudaStreamSynchronize(s);  // host vectors go out of scope
   if (!rc && e != cudaSuccess) rc = cuda_fail(e, "view upload");
   if (rc) {
@@ -1461,7 +1380,7 @@ void bsg_view_destroy(bsg_view *v) {
   if (!v) return;
   cudaSetDevice(v->h->device);
   cudaStreamSynchronize(v->h->stream);
-  void *ptrs[] = {v->d_row, v->d_col, v->d_center, v->d_scale, v->d_rows_unique, v->d_row_gather};
+  void *ptrs[] = {v->d_row, v->d_col, v->d_center, v->d_scale, v->d_rows_unique, v->d_row_gather, v->d_rowsel, v->d_colsel};
   for (void *p : ptrs)
     if (p) cudaFree(p);
   DevBuf *bufs[] = {&v->s_vec0, &v->s_vec1, &v->s_q0, &v->s_q1, &v->s_dig1, &v->s_dig2, &v->s_part, &v->s_scal,
@@ -1479,6 +1398,7 @@ int bsg_view_cprodvec_dev(bsg_view *v, const double *x_dev, double *out_dev, voi
   // ordered with the caller's kernels and collectives, not on the handle's private non-blocking stream
   cudaStream_t s = stream ? (cudaStream_t)stream : cudaStreamLegacy;
   if (v->nc == 0) return BSG_OK;
+  if (h->fbm_generic) return dosage_cprodvec(v, x_dev, out_dev, s);  // byte-operand kernel (bsg_dosage.cu)
   using namespace pmv;
   Scal *sc = v->s_scal.as<Scal>();
   // few missing values: the kernel runs in its no-missing mode and the N plane comes from the per-SNP lists
@@ -1722,6 +1642,28 @@ static bool use_T(const bsg_bed *h) {
 
 }  // extern "C"
 
+// Vector preparation of the byte-operand kernels (bsg_dosage.cu), in the format of the 2-bit kernels.  X.y: the digit blocks
+// of z = x / s (or x) over the selected columns in k_pmvT's step order, with the partials of C = sum c z.
+int bsg::dosage_prep_cols(bsg_view *v, const double *x_dev, cudaStream_t s) {
+  return prep_T(v, v->has_scaling ? 1 : 0, x_dev, v->d_center, v->d_scale, 1, nullptr, false, s);
+}
+
+// Xt.y: maximum and finiteness of x over the selected rows and its integer scatter by physical sample into Q (n entries,
+// zeroed here; an identity selection scatters to the same positions); the digit layout is written by bsg_dosage.cu.
+int bsg::dosage_prep_rows(bsg_view *v, const double *x_dev, long long *Q, cudaStream_t s) {
+  using namespace pmv;
+  Scal *sc = v->s_scal.as<Scal>();
+  BSG_CUDA(cudaMemsetAsync(sc, 0, sizeof(Scal), s));
+  k_prep1<<<SUMCZ_BLOCKS, 256, 0, s>>>(0, x_dev, nullptr, nullptr, v->nr, hb_bits(v->row_maxmult), sc);
+  count_launch();
+  BSG_CUDA(cudaMemsetAsync(Q, 0, (size_t)v->h->n * sizeof(long long), s));
+  k_quantise<<<launch_cap(std::max(v->nr, 1), 256, 592), 256, 0, s>>>(0, x_dev, nullptr, nullptr, v->nr,
+                                                                     v->row_identity ? nullptr : v->d_row, sc, 60, Q, nullptr);
+  count_launch();
+  BSG_CUDA(cudaGetLastError());
+  return BSG_OK;
+}
+
 // X~ x : lines = samples of copy B, contraction over SNP columns.  comm != null: the result is summed over the column
 // shards of the communicator (every rank receives the full n-vector).
 int bsg::view_prodvec_comm(bsg_view *v, const double *x_dev, double *out_dev, cudaStream_t s, bsg_comm *comm) {
@@ -1729,6 +1671,10 @@ int bsg::view_prodvec_comm(bsg_view *v, const double *x_dev, double *out_dev, cu
   bsg_bed *h = v->h;
   BSG_TRY(bind_device(h));
   if (v->nr == 0) return BSG_OK;
+  if (h->fbm_generic) {  // dosage FBM: byte-operand kernels over the value copy (bsg_dosage.cu), one device only
+    if (comm) return fail(BSG_ERR_ARG, "X.y summed over column shards needs hard calls; this handle holds dosages.");
+    return dosage_prodvec(v, x_dev, out_dev, s);
+  }
   if (use_T(h)) return prodvec_T(v, x_dev, out_dev, s, comm);  // transposing kernel over the SNP-major copy
   using namespace pmv;
   Scal *sc = v->s_scal.as<Scal>();
@@ -1783,7 +1729,11 @@ static int view_host_call(bsg_view *v, const double *x, double *out, bool cprod)
     BSG_CUDA(cudaMemcpyAsync(&bad, &v->s_scal.as<pmv::Scal>()->nonfinite, sizeof(int), cudaMemcpyDeviceToHost, s));
   BSG_CUDA(cudaMemcpyAsync(out, dout, (size_t)nout * sizeof(double), cudaMemcpyDeviceToHost, s));
   BSG_CUDA(cudaStreamSynchronize(s));
-  if (bad) {
+  if (bad && h->fbm_generic) {  // dosages: the literal per-element fp64 loop over code256[byte]
+    BSG_TRY(dosage_literal(v, cprod, dx, dout, s));
+    BSG_CUDA(cudaMemcpyAsync(out, dout, (size_t)nout * sizeof(double), cudaMemcpyDeviceToHost, s));
+    BSG_CUDA(cudaStreamSynchronize(s));
+  } else if (bad) {
     BSG_TRY(cprod ? simple_cprodvec(h, v->d_row, v->nr, v->d_col, v->nc, v->d_center, v->d_scale, dx, dout, s)
                   : simple_prodvec(h, v->d_row, v->nr, v->d_col, v->nc, v->d_center, v->d_scale, dx, dout, s));
     BSG_CUDA(cudaMemcpyAsync(out, dout, (size_t)nout * sizeof(double), cudaMemcpyDeviceToHost, s));
@@ -2087,6 +2037,7 @@ __global__ void k_counts_from_planes(int nr, int nc, const double *__restrict__ 
 }
 
 int row_counts_planes(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, int nc, int32_t *d_out4) {
+  BSG_PACKED_ONLY(h, "Counts by row");
   bsg_view *v = nullptr;
   BSG_TRY(cached_view(h, ind_row, nr, ind_col, nc, nullptr, nullptr, &v));
   cudaStream_t s = h->stream;
@@ -2120,6 +2071,7 @@ int bsg_prod_and_rowsumssq(bsg_bed *h, const int *ind_row, int nr, const int *in
   if (!h || !XV || !rowSumsSq || (!V && K > 0)) return fail(BSG_ERR_ARG, "null argument");
   if (!center || !scale) return fail(BSG_ERR_DIM, "Incompatibility between dimensions.");
   if (K < 0) return fail(BSG_ERR_ARG, "negative length");
+  BSG_PACKED_ONLY(h, "prod_and_rowSumsSq");
   bsg_view *v = nullptr;
   BSG_TRY(cached_view(h, ind_row, nr, ind_col, nc, center, scale, &v));
   nr = v->nr;
@@ -2209,6 +2161,58 @@ int bsg_prod_and_rowsumssq(bsg_bed *h, const int *ind_row, int nr, const int *in
     }
   }
   if (need_simple) BSG_TRY(simple_rowsumssq(h, v->d_row, nr, v->d_col, nc, v->d_center, v->d_scale, d_rs, s));
+  BSG_CUDA(cudaMemcpyAsync(XV, dXV, (size_t)nr * K * sizeof(double), cudaMemcpyDeviceToHost, s));
+  BSG_CUDA(cudaMemcpyAsync(rowSumsSq, d_rs, (size_t)nr * sizeof(double), cudaMemcpyDeviceToHost, s));
+  BSG_CUDA(cudaStreamSynchronize(s));
+  return BSG_OK;
+}
+
+// prod_and_rowSumsSq2 (src/project-utils.cpp:11-43, snp_projectSelfPCA): the same two outputs for an FBM.code256 handle
+// with the accessor's literal semantics, x = (code256[b] - c_j) / s_j with an NA code giving NA_real.  XV = K single-vector
+// X.y passes (the byte-operand kernels on a dosage handle, the 2-bit kernels on hard calls), then every row holding an
+// NA code in a selected column is NaN.  rowSumsSq: one literal fp64 pass over the codes (k_proj_literal), which also
+// flags those rows.  Non-finite x, center or 1/scale: XV is recomputed by the same literal pass.
+int bsg_prod_and_rowsumssq2(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, int nc, const double *center,
+                            const double *scale, const double *V, int K, double *XV, double *rowSumsSq) {
+  if (!h || !XV || !rowSumsSq || (!V && K > 0)) return fail(BSG_ERR_ARG, "null argument");
+  if (!center || !scale) return fail(BSG_ERR_DIM, "Incompatibility between dimensions.");
+  if (K < 0) return fail(BSG_ERR_ARG, "negative length");
+  if (h->kind != BSG_KIND_FBM)
+    return fail(BSG_ERR_TYPE, "prod_and_rowSumsSq2 takes an FBM.code256 handle (a .bed handle: prod_and_rowSumsSq).");
+  if (!h->dos_scale) BSG_PACKED_ONLY(h, "prod_and_rowSumsSq2");
+  bsg_view *v = nullptr;
+  BSG_TRY(cached_view(h, ind_row, nr, ind_col, nc, center, scale, &v));
+  nr = v->nr;
+  nc = v->nc;
+  if (nr == 0) return BSG_OK;
+  cudaStream_t s = h->stream;
+  ProjScratch mem{h};
+  double *dV = nullptr, *dXV = nullptr, *d_rs = nullptr;
+  uint8_t *d_na = nullptr;
+  int *d_bad = nullptr;
+  BSG_TRY(mem.alloc(&dV, (size_t)nc * K));
+  BSG_TRY(mem.alloc(&dXV, (size_t)nr * K));
+  BSG_TRY(mem.alloc(&d_rs, (size_t)nr));
+  BSG_TRY(mem.alloc(&d_na, (size_t)nr));
+  BSG_TRY(mem.alloc(&d_bad, 1));
+  BSG_CUDA(cudaMemsetAsync(d_bad, 0, sizeof(int), s));
+  if (K > 0) BSG_CUDA(cudaMemcpyAsync(dV, V, (size_t)nc * K * sizeof(double), cudaMemcpyHostToDevice, s));
+  for (int k = 0; k < K && nc > 0; k++) {
+    BSG_TRY(bsg_view_prodvec_dev(v, dV + (size_t)k * nc, dXV + (size_t)k * nr, s));
+    k_or_flag<<<1, 1, 0, s>>>(v->s_scal.as<pmv::Scal>(), d_bad);
+    count_launch();
+  }
+  if (nc == 0 && K > 0) BSG_CUDA(cudaMemsetAsync(dXV, 0, (size_t)nr * K * sizeof(double), s));
+  BSG_TRY(fbm_proj_literal(v, dV, 0, nullptr, d_rs, d_na, s));
+  int bad = 0;
+  BSG_CUDA(cudaMemcpyAsync(&bad, d_bad, sizeof(int), cudaMemcpyDeviceToHost, s));
+  BSG_CUDA(cudaStreamSynchronize(s));
+  if (bad) {  // the reference's per-element Inf / NaN
+    BSG_CUDA(cudaMemsetAsync(dXV, 0, (size_t)nr * K * sizeof(double), s));
+    BSG_TRY(fbm_proj_literal(v, dV, K, dXV, d_rs, d_na, s));
+  } else {
+    BSG_TRY(fbm_nan_rows(d_na, nr, K, dXV, s));
+  }
   BSG_CUDA(cudaMemcpyAsync(XV, dXV, (size_t)nr * K * sizeof(double), cudaMemcpyDeviceToHost, s));
   BSG_CUDA(cudaMemcpyAsync(rowSumsSq, d_rs, (size_t)nr * sizeof(double), cudaMemcpyDeviceToHost, s));
   BSG_CUDA(cudaStreamSynchronize(s));

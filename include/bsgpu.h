@@ -78,6 +78,23 @@ int bsg_open_synth_ld(int n, int m, uint64_t seed, double na_rate, int64_t col_o
  * src/colstats.cpp:8-35, src/corr.cpp:113-118, src/ld-scores.cpp:93-96). */
 int bsg_open_fbm256(const uint8_t *bytes, int n, int m, const double *code256, int device, int layouts,
                     bsg_bed **out);
+/* Dosage tables.  An FBM.code256 whose codes are not 0 / 1 / 2 / NA stages as a generic handle.  It is also a DOSAGE
+ * handle when some integer D in 1..255 makes D * v an integer in 0..255 (within 1e-9) for every finite code value v, and
+ * every other code value is NaN: CODE_DOSAGE (R/bigSNP-class.R:13: 0, 1, 2, NA, 0, 1, 2, seq(0, 2, by = 0.01), NA x 48)
+ * gives D = 100.  bsg_code256_dosage_scale returns the smallest such D, or 0.  Dosage handles also serve X.y and Xt.y
+ * (bsg_prodvec, bsg_cprodvec, views), bsg_prod_and_rowsumssq2 and bsg_randomsvd with explicit center / scale
+ * (bsg_colstats, behind the NULL default, needs hard calls), on the integer tensor pipe: round(D v) is an exact byte, the sums are exact integers.
+ *   - Element (bigstatsr's SubBMCode256Acc and scaling, [bigstatsr, unvendored]): (code256[b] - c_j) / s_j.
+ *   - An NA code is NA_real and poisons every output it touches, even against a zero weight: X.y rows holding an NA in a
+ *     selected column and Xt.y columns holding an NA in a selected row are NaN.  (.bed handles differ: there a missing
+ *     value counts as 0 after centering, src/bed-acc.h:98-111.)
+ *   - Non-finite x, center or 1/scale: as for .bed handles, the _dev forms return all NaN and the host forms re-run a
+ *     literal per-element fp64 loop that propagates Inf / NaN element by element.
+ *   - Footprint: the first product builds a value copy (round_up(n, 128) bytes per SNP) next to the raw bytes and the
+ *     2-bit copy: about 2 n m + n m / 4 bytes in all (50,000 x 600,000: 67 GB).  One device; no column shards.
+ * bsg_dosage_scale(h) is the handle's D (0: hard calls, or a table that does not qualify). */
+int bsg_code256_dosage_scale(const double code256[256]);
+int bsg_dosage_scale(const bsg_bed *h);
 void bsg_close(bsg_bed *h);
 int bsg_nrow(const bsg_bed *h);
 int bsg_ncol(const bsg_bed *h);
@@ -177,6 +194,14 @@ int bsg_set_prodvec_path(int path);
 int bsg_prod_and_rowsumssq(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, int nc,
                            const double *center, const double *scale, const double *V, int K,
                            double *XV, double *rowSumsSq);
+/* _bigsnpr_prod_and_rowSumsSq2: src/project-utils.cpp:11-43 (R: part_prod2 of snp_projectSelfPCA, R/bed-projectPCA.R:252-281).
+ * Same outputs for an FBM.code256 handle (hard calls or a dosage table, bsg_dosage_scale > 0) with the accessor's literal
+ * semantics: x = (code256[b] - c_j) / s_j and an NA code is NA_real, so a row holding an NA code in a selected column
+ * has NaN in XV and in rowSumsSq.  XV runs on the integer tensor pipe (K single-vector X.y passes); rowSumsSq is one
+ * literal fp64 pass over the codes (x^2 is not linear in the code), not a tuned path.  Other handles: BSG_ERR_TYPE. */
+int bsg_prod_and_rowsumssq2(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, int nc,
+                            const double *center, const double *scale, const double *V, int K,
+                            double *XV, double *rowSumsSq);
 /* _bigsnpr_multLinReg: src/multLinReg.cpp:8-88 (R: pcadapt0, R/pcadapt.R:3-27).  U is nr x K column-major;
  * tscores is nc x K column-major (the reference returns transpose(res)); NA_REAL is written as NaN.
  * Works on .bed handles and on FBM.code256 handles alike (the reference dispatches on the class, :72-92). */

@@ -330,6 +330,22 @@ SEXP _bigsnpr_prod_and_rowSumsSq(SEXP obj_bed, SEXP ind_row, SEXP ind_col, SEXP 
   return res;
 }
 
+/* _bigsnpr_prod_and_rowSumsSq2: src/project-utils.cpp:11-43 (6 arguments; `BM` is an FBM.code256 environment, hard calls
+ * or a dosage table) -> list(XV, rowSumsSq); a row holding an NA code in a selected column is NaN (NA_real in the reference) */
+SEXP _bigsnpr_prod_and_rowSumsSq2(SEXP BM, SEXP ind_row, SEXP ind_col, SEXP center, SEXP scale, SEXP V) {
+  bsg_bed *h = fbm_handle_of(BM);
+  int nr = LENGTH(ind_row), nc = LENGTH(ind_col), K = Rf_ncols(V);
+  if (LENGTH(center) != nc || LENGTH(scale) != nc || Rf_nrows(V) != nc) Rf_error("Incompatibility between dimensions.");
+  SEXP XV = PROTECT(Rf_allocMatrix(REALSXP, nr, K)), rss = PROTECT(Rf_allocVector(REALSXP, nr));
+  chk(bsg_prod_and_rowsumssq2(h, INTEGER(ind_row), nr, INTEGER(ind_col), nc, REAL(center), REAL(scale), REAL(V), K,
+                              REAL(XV), REAL(rss)));
+  SEXP res = PROTECT(Rf_allocVector(VECSXP, 2));
+  SET_VECTOR_ELT(res, 0, XV);
+  SET_VECTOR_ELT(res, 1, rss);
+  UNPROTECT(3);
+  return res;
+}
+
 /* _bigsnpr_multLinReg: src/multLinReg.cpp:64-88 (5 arguments; `obj` is a bed or an FBM.code256 environment) */
 SEXP _bigsnpr_multLinReg(SEXP obj, SEXP ind_row, SEXP ind_col, SEXP U, SEXP ncores) {
   bsg_bed *h = any_handle(obj); /* src/multLinReg.cpp:72-78: FBM.code256 or bed, else "Unknown object type." */
@@ -353,8 +369,10 @@ SEXP _bigsnpr_bed_tcrossprod_gpu(SEXP obj_bed, SEXP ind_row, SEXP ind_col, SEXP 
   return K;
 }
 
+/* `obj_bed` may also be an FBM.code256 environment (big_randomSVD's branch of snp_autoSVD passes G): a dosage table needs
+ * center / scale (snp_scaleBinom); NULL scaling (bed_scaleBinom) needs hard calls */
 SEXP _bigsnpr_bed_randomSVD_gpu(SEXP obj_bed, SEXP ind_row, SEXP ind_col, SEXP center, SEXP scale, SEXP k, SEXP tol) {
-  bsg_bed *h = handle_of(obj_bed);
+  bsg_bed *h = any_handle(obj_bed);
   int nr = LENGTH(ind_row), nc = LENGTH(ind_col), kk = Rf_asInteger(k), niter = 0, nops = 0;
   SEXP d = PROTECT(Rf_allocVector(REALSXP, kk)), u = PROTECT(Rf_allocMatrix(REALSXP, nr, kk));
   SEXP v = PROTECT(Rf_allocMatrix(REALSXP, nc, kk));
@@ -450,6 +468,7 @@ static const R_CallMethodDef CallEntries[] = {
     {"_bigsnpr_readbina2", (DL_FUNC)&_bigsnpr_readbina2, 5},
     {"_bigsnpr_writebina", (DL_FUNC)&_bigsnpr_writebina, 5},
     {"_bigsnpr_prod_and_rowSumsSq", (DL_FUNC)&_bigsnpr_prod_and_rowSumsSq, 6},
+    {"_bigsnpr_prod_and_rowSumsSq2", (DL_FUNC)&_bigsnpr_prod_and_rowSumsSq2, 6},
     {"_bigsnpr_multLinReg", (DL_FUNC)&_bigsnpr_multLinReg, 5},
     {"_bigsnpr_bed_tcrossprod_gpu", (DL_FUNC)&_bigsnpr_bed_tcrossprod_gpu, 5},
     {"_bigsnpr_bed_randomSVD_gpu", (DL_FUNC)&_bigsnpr_bed_randomSVD_gpu, 7},
