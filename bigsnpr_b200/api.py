@@ -847,6 +847,97 @@ def snp_clumping(G, infos_chr, ind_row=..., S=None, thr_r2=0.2, size=None, infos
     return np.sort(np.concatenate(kept)) if kept else np.zeros(0, dtype=np.int32)
 
 
+def clumping_chr_cached(G, keep, sqcor, spInd, rowInd, colInd, ordInd, rankInd, pos, sumX, denoX, size, thr, ncores=1):
+    """src/clumping-cached.cpp:11-110: writes 0 / 1 into `keep` (int32, one per column of colInd) and returns `sqcor` as
+    passed.  The reference's r2 cache never changes a decision, so the call is clumping_chr's (bsg_clumping_chr_fbm)."""
+    if np.asarray(spInd).size != np.asarray(colInd).size:
+        raise ValueError(ERROR_DIM)
+    keep[:] = clumping_chr(G, rowInd, colInd, ordInd, rankInd, pos, sumX, denoX, size, thr, ncores)
+    return sqcor
+
+
+class GridClumping(list):
+    """snp_grid_clumping's result: one list per chromosome of 1-based index arrays, with the `grid` attribute (dict of
+    columns size, thr_r2, grp_num, thr_imp, one row per keep set of a chromosome)."""
+
+    grid = None
+
+
+def _order_decreasing(x):
+    """R's order(x, decreasing = TRUE): ties by position, NA last."""
+    x = np.asarray(x, dtype=np.float64)
+    key = np.where(np.isnan(x), np.inf, -x)
+    return np.argsort(key, kind="stable")
+
+
+def snp_grid_clumping(G, infos_chr, infos_pos, lpS, ind_row=..., grid_thr_r2=(0.01, 0.05, 0.1, 0.2, 0.5, 0.8, 0.95),
+                      grid_base_size=(50, 100, 200, 500), infos_imp=None, grid_thr_imp=1, groups=None, exclude=None,
+                      ncores=1):
+    """Grid of clumping (R/SCT.R:32-151) on an FBM.code256 handle: for every chromosome, every (thr_imp, group) subset and
+    every (thr_r2, base_size) point, the indices kept by clumping_chr with size 1000 * base_size / thr_r2 bp.  One
+    bsg_grid_clumping_chr call per chromosome computes each pair's statistic once and resolves every instance together."""
+    _assert_bed(G)
+    cols = G.cols_along()
+    infos_chr = np.asarray(infos_chr)
+    infos_imp = np.ones(cols.size) if infos_imp is None else _f64(infos_imp)
+    for v in (infos_chr, infos_pos, infos_imp, lpS):
+        _assert_lengths(v, cols)
+    infos_pos, lpS = _f64(infos_pos), _f64(lpS)
+    if groups is None:
+        groups = [cols]
+    if not isinstance(groups, (list, tuple)):
+        raise TypeError("'groups' is not of class 'list'.")
+    groups = [np.asarray(gr, dtype=np.int64).reshape(-1) for gr in groups]
+    ind_row = G.rows_along() if ind_row is ... else _i32(ind_row)
+    THR_IMP = np.unique(np.asarray(grid_thr_imp, dtype=np.float64).reshape(-1))
+    THR_CLMP = np.unique(np.asarray(grid_thr_r2, dtype=np.float64).reshape(-1))
+    BASE = np.unique(np.asarray(grid_base_size, dtype=np.float64).reshape(-1))
+    # expand.grid(size, thr.r2, grp.num, thr.imp): the first factor varies fastest
+    g_imp, g_grp, g_thr, g_size = (a.ravel() for a in np.meshgrid(THR_IMP, np.arange(1, len(groups) + 1), THR_CLMP, BASE,
+                                                                   indexing="ij"))
+    grid = {"size": np.trunc(g_size / g_thr).astype(np.int32), "thr_r2": g_thr, "grp_num": g_grp.astype(np.int32),
+            "thr_imp": g_imp}
+    # the points of one subset, in the order of the reference's loops (thr.r2 outer, base.size inner)
+    p_thr, p_base = (a.ravel() for a in np.meshgrid(THR_CLMP, BASE, indexing="ij"))
+    p_size = 1000 * p_base / p_thr  # R/SCT.R:133, in bp
+    npt = p_thr.size
+    excl = np.asarray([] if exclude is None else exclude, dtype=np.int64)
+    noexcl = np.arange(1, infos_chr.size + 1)
+    noexcl = noexcl[~np.isin(noexcl, excl)]
+    out = GridClumping()
+    for chrom in sorted(set(infos_chr[noexcl - 1].tolist())):
+        ind_chr = noexcl[infos_chr[noexcl - 1] == chrom].astype(np.int32)
+        pos_chr = infos_pos[ind_chr - 1]
+        st = snp_colstats(G, ind_row, ind_chr, ncores)
+        if np.any(np.diff(pos_chr) < 0):
+            raise ValueError("'pos.chr' is not sorted.")
+        info_chr, S_chr = infos_imp[ind_chr - 1], lpS[ind_chr - 1]
+        cur = np.arange(ind_chr.size)  # positions within ind_chr that pass the thresholds of imputation so far
+        sub_cols, sub_ords = [], []
+        for thr_imp in THR_IMP:
+            cur = cur[info_chr[cur] >= thr_imp]
+            for group in groups:
+                sub = cur[np.isin(ind_chr[cur], group)]
+                sub_cols.append(sub)
+                sub_ords.append(_order_decreasing(S_chr[sub]))
+        lens = _i32([s.size for s in sub_cols])
+        cat = lambda parts: _i32(np.concatenate(parts) + 1) if parts else np.zeros(0, dtype=np.int32)  # noqa: E731
+        keep = np.full(max(int(lens.sum()) * npt, 1), -1, dtype=np.int32)
+        check(lib().bsg_grid_clumping_chr(G._h, _pi(ind_row), ind_row.size, _pi(ind_chr), ind_chr.size, _pd(_f64(pos_chr)),
+                                          _pd(_f64(st["sumX"])), _pd(_f64(st["denoX"])), len(sub_cols), _pi(lens),
+                                          _pi(cat(sub_cols)), _pi(cat(sub_ords)), npt, _pd(_f64(p_thr)), _pd(_f64(p_size)),
+                                          _pi(keep)))
+        res, o = [], 0
+        for sub in sub_cols:
+            for _ in range(npt):
+                k = keep[o:o + sub.size]
+                res.append(ind_chr[sub[k == 1]])
+                o += sub.size
+        out.append(res)
+    out.grid = grid
+    return out
+
+
 def prod_and_rowSumsSq(obj_bed, ind_row, ind_col, center, scale, V):
     """src/bed-fun.cpp:103-133 -> (XV (nr, K), rowSumsSq (nr)); V has one row per selected column (:116)."""
     ind_row, ind_col = _i32(ind_row), _i32(ind_col)

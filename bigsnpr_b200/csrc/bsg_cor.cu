@@ -330,7 +330,8 @@ __global__ void k_cor_from_sums(const int *__restrict__ sums, const Tile *__rest
                                 const int *__restrict__ wlen, const long long *__restrict__ boff,
                                 const int32_t *__restrict__ cnt, int nrow, int npad, const double *__restrict__ thr,
                                 double *__restrict__ band, uint8_t *__restrict__ keep, int tn,
-                                const double *__restrict__ center, const double *__restrict__ scale, double thr_r2) {
+                                const double *__restrict__ center, const double *__restrict__ scale, double thr_r2,
+                                int nlev) {
   const long long first = boff[j0_begin], total = boff[j0_end] - first;
   for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < total; t += (long long)gridDim.x * blockDim.x) {
     // locate j0 by binary search on boff
@@ -366,13 +367,20 @@ __global__ void k_cor_from_sums(const int *__restrict__ sums, const Tile *__rest
       xySum = (double)aa;
     }
     (void)nona_d;
-    if (KIND == 3) {
+    if (KIND == 3 || KIND == 4) {
       // clumping_chr on an FBM.code256 (src/clumping.cpp:66-73): no missing-value handling in the reference -- a
       // missing genotype makes xySum NA and `r2 > thr` false; `center` / `scale` carry the caller's sumX / denoX
       const bool has_na = cnt[4 * (int64_t)j0 + 3] != 0 || cnt[4 * (int64_t)j + 3] != 0;
       const double num = xySum - center[j] * center[j0] / nrow;
       const double r2 = num * num / (scale[j] * scale[j0]);
-      keep[o] = (!has_na && r2 > thr_r2) ? 1 : 0;
+      if (KIND == 3) {
+        keep[o] = (!has_na && r2 > thr_r2) ? 1 : 0;
+      } else {  // snp_grid_clumping: how many of the sorted thresholds thr[0..nlev) r2 exceeds
+        int l = 0;
+        if (!has_na)
+          for (int t = 0; t < nlev; t++) l += r2 > thr[t];
+        keep[o] = (uint8_t)l;
+      }
       continue;
     }
     if (KIND == 2) {
@@ -492,10 +500,10 @@ struct CorScratch {
   bool own_M = true;  // false: M aliases the handle's SNP-major copy (identity rows and columns)
   int *wlen = nullptr, *reach = nullptr;
   long long *boff = nullptr;
-  double *thr = nullptr, *band = nullptr, *res = nullptr;
+  double *thr = nullptr, *band = nullptr, *res = nullptr, *lev = nullptr;
   uint8_t *keep = nullptr;
   ~CorScratch() {
-    void *p[] = {own_M ? M : nullptr, wlen, reach, boff, thr, band, res, keep};
+    void *p[] = {own_M ? M : nullptr, wlen, reach, boff, thr, band, res, lev, keep};
     for (void *q : p)
       if (q) cudaFree(q);
   }
@@ -505,6 +513,8 @@ struct ClumpParams {
   const double *center = nullptr, *scale = nullptr;  // host, per selected column (fbm: sumX / denoX)
   double thr = 0;
   bool fbm = false;  // src/clumping.cpp's statistic instead of src/clumping-bed.cpp's
+  const double *levels = nullptr;  // host, nlev sorted thresholds: keep[] receives how many r2 exceeds (fbm only)
+  int nlev = 0;
 };
 
 static int cor_common(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, int nc, double size,
@@ -532,6 +542,17 @@ static int cor_common(bsg_bed *h, const int *ind_row, int nr, const int *ind_col
       sc.thr = d_sx;  // owned by the scratch (freed with it)
       sc.res = d_dx;
       BSG_CUDA(pool_alloc((void **)&sc.keep, tot, h->device, s));
+      if (clump->levels) {
+        BSG_TRY(to_dev(&sc.lev, std::vector<double>(clump->levels, clump->levels + clump->nlev), s));
+        if (h->dos_scale > 0)  // exact integer pair sums of the D-scaled bytes (bsg_grid.cu)
+          BSG_TRY(dosage_pair_levels(h, d_row, nr, d_col, nc, w.wlen, sc.wlen, sc.boff, d_sx, d_dx, sc.lev, clump->nlev,
+                                     sc.keep, s));
+        else
+          BSG_TRY(generic_pairs(h, d_row, nr, d_col, nc, 4, sc.wlen, sc.boff, w.total, sc.lev, nullptr, sc.keep, d_sx, d_dx,
+                                (double)clump->nlev, s));
+        BSG_CUDA(cudaStreamSynchronize(s));
+        return BSG_OK;
+      }
     } else {
       BSG_CUDA(pool_alloc((void **)&sc.band, tot * sizeof(double), h->device, s));
       if (!ld) {
@@ -579,6 +600,7 @@ static int cor_common(bsg_bed *h, const int *ind_row, int nr, const int *ind_col
     BSG_TRY(to_dev(&d_cs, sv, s));
     sc.thr = d_cc;   // owned by the scratch (freed with it)
     sc.res = d_cs;
+    if (clump->levels) BSG_TRY(to_dev(&sc.lev, std::vector<double>(clump->levels, clump->levels + clump->nlev), s));
     BSG_CUDA(pool_alloc((void **)&sc.keep, (size_t)(w.total ? w.total : 1), h->device, s));
   } else {
     BSG_CUDA(pool_alloc((void **)&sc.band, (size_t)(w.total ? w.total : 1) * sizeof(double), h->device, s));
@@ -707,18 +729,21 @@ static int cor_common(bsg_bed *h, const int *ind_row, int nr, const int *ind_col
       }
       const long long npairs = w.boff[j0_end] - w.boff[j0_begin];
       const int eg = (int)std::min<long long>((npairs + 255) / 256, 132 * 16);
-      if (clump && clump->fbm)
+      if (clump && clump->levels)
+        k_cor_from_sums<4><<<eg, 256, 0, s>>>(d_sums, d_tiles, d_rbs, ib_start, j0_begin, j0_end, sc.wlen, sc.boff, d_cnt, nr,
+                                              npad, sc.lev, nullptr, sc.keep, TNv, d_cc, d_cs, 0.0, clump->nlev);
+      else if (clump && clump->fbm)
         k_cor_from_sums<3><<<eg, 256, 0, s>>>(d_sums, d_tiles, d_rbs, ib_start, j0_begin, j0_end, sc.wlen, sc.boff, d_cnt, nr,
-                                              npad, nullptr, nullptr, sc.keep, TNv, d_cc, d_cs, clump->thr);
+                                              npad, nullptr, nullptr, sc.keep, TNv, d_cc, d_cs, clump->thr, 0);
       else if (clump)
         k_cor_from_sums<2><<<eg, 256, 0, s>>>(d_sums, d_tiles, d_rbs, ib_start, j0_begin, j0_end, sc.wlen, sc.boff, d_cnt, nr,
-                                              npad, nullptr, nullptr, sc.keep, TNv, d_cc, d_cs, clump->thr);
+                                              npad, nullptr, nullptr, sc.keep, TNv, d_cc, d_cs, clump->thr, 0);
       else if (ld)
         k_cor_from_sums<1><<<eg, 256, 0, s>>>(d_sums, d_tiles, d_rbs, ib_start, j0_begin, j0_end, sc.wlen, sc.boff, d_cnt, nr,
-                                              npad, nullptr, sc.band, nullptr, TNv, nullptr, nullptr, 0.0);
+                                              npad, nullptr, sc.band, nullptr, TNv, nullptr, nullptr, 0.0, 0);
       else
         k_cor_from_sums<0><<<eg, 256, 0, s>>>(d_sums, d_tiles, d_rbs, ib_start, j0_begin, j0_end, sc.wlen, sc.boff, d_cnt, nr,
-                                              npad, sc.thr, sc.band, sc.keep, TNv, nullptr, nullptr, 0.0);
+                                              npad, sc.thr, sc.band, sc.keep, TNv, nullptr, nullptr, 0.0, 0);
       count_launch(2);
       cudaError_t e2 = cudaStreamSynchronize(s);
       cudaFree(d_tiles);
@@ -728,6 +753,33 @@ static int cor_common(bsg_bed *h, const int *ind_row, int nr, const int *ind_col
     }
   }
   BSG_CUDA(cudaGetLastError());
+  return BSG_OK;
+}
+
+LevelBand::~LevelBand() {
+  void *p[] = {d_wlen, d_boff, d_lev};
+  for (void *q : p)
+    if (q) cudaFree(q);
+}
+
+int level_band(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, int nc, double size, const double *pos,
+               const double *sumX, const double *denoX, const double *levels, int nlev, LevelBand &b) {
+  Window w;
+  CorScratch sc;
+  ClumpParams cp;
+  cp.center = sumX;
+  cp.scale = denoX;
+  cp.fbm = true;
+  cp.levels = levels;
+  cp.nlev = nlev;
+  BSG_TRY(cor_common(h, ind_row, nr, ind_col, nc, size, pos, nullptr, false, w, sc, &cp));
+  BSG_CUDA(cudaStreamSynchronize(h->stream));
+  b.wlen.swap(w.wlen);
+  b.boff.swap(w.boff);
+  b.total = w.total;
+  std::swap(b.d_wlen, sc.wlen);  // the band and its offsets outlive the scratch
+  std::swap(b.d_boff, sc.boff);
+  std::swap(b.d_lev, sc.keep);
   return BSG_OK;
 }
 

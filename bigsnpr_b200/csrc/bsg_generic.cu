@@ -62,7 +62,7 @@ __global__ void k_pairs(const uint8_t *__restrict__ raw, int64_t n_tot, const do
     }
     const int j0 = lo, j = j0 - 1 - (int)(o - boff[j0]);
     const uint8_t *cx = raw + (int64_t)(cols ? cols[j0] : j0) * n_tot, *cy = raw + (int64_t)(cols ? cols[j] : j) * n_tot;
-    if (KIND == 3) {
+    if (KIND == 3 || KIND == 4) {
       // xySum with the accessor's values (NA_real for a missing code: the sum and r2 are NA, never > thr)
       double xy = 0;
       for (int i = lane; i < nr; i += 32) {
@@ -73,7 +73,13 @@ __global__ void k_pairs(const uint8_t *__restrict__ raw, int64_t n_tot, const do
       if (lane == 0) {
         const double num = xy - sumX[j] * sumX[j0] / nr;
         const double r2 = num * num / (denoX[j] * denoX[j0]);
-        keep[o] = (r2 > thr_r2) ? 1 : 0;  // false for NaN
+        if (KIND == 3) {
+          keep[o] = (r2 > thr_r2) ? 1 : 0;  // false for NaN
+        } else {  // level: how many of the (int)thr_r2 sorted thresholds thr[] r2 exceeds
+          int l = 0;
+          for (int t = 0; t < (int)thr_r2; t++) l += r2 > thr[t];
+          keep[o] = (uint8_t)l;
+        }
       }
       continue;
     }
@@ -171,6 +177,8 @@ int generic_pairs(bsg_bed *h, const int *d_row, int nr, const int *d_col, int nc
     gen::k_pairs<0><<<grid, 256, 0, s>>>(h->raw, h->n, c3, h->d_code, d_row, nr, d_col, nc, d_wlen, d_boff, total, d_thr, d_band, d_keep, d_sumX, d_denoX, thr_r2);
   else if (kind == 1)
     gen::k_pairs<1><<<grid, 256, 0, s>>>(h->raw, h->n, c3, h->d_code, d_row, nr, d_col, nc, d_wlen, d_boff, total, d_thr, d_band, d_keep, d_sumX, d_denoX, thr_r2);
+  else if (kind == 4)
+    gen::k_pairs<4><<<grid, 256, 0, s>>>(h->raw, h->n, c3, h->d_code, d_row, nr, d_col, nc, d_wlen, d_boff, total, d_thr, d_band, d_keep, d_sumX, d_denoX, thr_r2);
   else
     gen::k_pairs<3><<<grid, 256, 0, s>>>(h->raw, h->n, c3, h->d_code, d_row, nr, d_col, nc, d_wlen, d_boff, total, d_thr, d_band, d_keep, d_sumX, d_denoX, thr_r2);
   count_launch();

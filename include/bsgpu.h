@@ -215,6 +215,20 @@ int bsg_clumping_chr_fbm(bsg_bed *h, const int *ind_row, int nr, const int *ind_
                          const double *denoX, const int *ordInd, const double *pos, double size, double thr,
                          int *keep);
 
+/* snp_grid_clumping, one chromosome (R/SCT.R:32-151): every clumping_chr_cached call of the chromosome in one call.
+ * ind_col (nc columns after `exclude`) with sorted pos and the snp_colstats vectors sumX / denoX over ind_row.
+ * nsub subsets, concatenated: subset s has sub_len[s] entries of sub_col (1-based positions within ind_col, strictly
+ * ascending) and of sub_ord (1-based positions within the subset by decreasing priority: order(S, decreasing = TRUE)).
+ * npt grid points (thr_r2[p], size_bp[p]); size_bp is the reference's 1000 * base.size / thr.r2, in bp.
+ * keep (sum_s npt * sub_len[s] ints) receives, subset by subset, point by point, 0 / 1 per subset column: the keep
+ * vector of clumping_chr on that subset with that size and threshold.  The pair statistic of clumping_chr (bsg_clumping_chr_fbm)
+ * is computed once per pair at the largest size: hard calls on the Gram tiles, dosage handles (bsg_dosage_scale D > 0)
+ * as exact integer sums of D-scaled bytes on the tensor pipe (xySum = S / D^2), other tables by the fp64 kernels.
+ * At most 255 distinct thresholds; unsorted pos, a subset out of order or out of range: BSG_ERR_ARG. */
+int bsg_grid_clumping_chr(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, int nc, const double *pos,
+                          const double *sumX, const double *denoX, int nsub, const int *sub_len, const int *sub_col,
+                          const int *sub_ord, int npt, const double *thr_r2, const double *size_bp, int *keep);
+
 /* ---- Gram product --------------------------------------------------------------------------------- */
 /* bed_tcrossprodSelf's block loop collapsed into one call: R/bed-tcrossprodSelf.R:38-49 +
  * src/bed-mat-acc.cpp:30-49.  K is nr x nr; center/scale are the per-column scaling (length nc). */

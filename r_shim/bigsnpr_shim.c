@@ -294,6 +294,27 @@ SEXP _bigsnpr_clumping_chr(SEXP BM, SEXP BM2, SEXP rowInd, SEXP colInd, SEXP ord
   return R_NilValue;
 }
 
+/* _bigsnpr_clumping_chr_cached: src/clumping-cached.cpp:11-110 (14 arguments; one grid point of snp_grid_clumping,
+ * R/SCT.R:121-135).  keep goes into BM2 as for _bigsnpr_clumping_chr.  The reference's sparse r2 cache never changes a
+ * decision (a pair's r2 is the same whenever it is computed), so sqcor is returned as passed: R/SCT.R subsets it and hands it
+ * back, which is valid for any cache value.  spInd and rankInd (implied by ordInd) are not needed. */
+SEXP _bigsnpr_clumping_chr_cached(SEXP BM, SEXP BM2, SEXP sqcor, SEXP spInd, SEXP rowInd, SEXP colInd, SEXP ordInd,
+                                  SEXP rankInd, SEXP pos, SEXP sumX, SEXP denoX, SEXP size, SEXP thr, SEXP ncores) {
+  bsg_bed *h = fbm_handle_of(BM);
+  int nr = LENGTH(rowInd), nc = LENGTH(colInd);
+  if (LENGTH(spInd) != nc) Rf_error("Incompatibility between dimensions.");  /* myassert_size(spInd.size(), m) */
+  if (LENGTH(sumX) != nc || LENGTH(denoX) != nc || LENGTH(pos) != nc || LENGTH(ordInd) != nc)
+    Rf_error("Incompatibility between dimensions.");
+  size_t bytes = 0;
+  int *keep = (int *)fbm_map(BM2, sizeof(int), 1, &bytes);
+  if (bytes < (size_t)nc * sizeof(int)) { fbm_unmap(keep, bytes, 1); Rf_error("Incompatibility between dimensions."); }
+  int rc = bsg_clumping_chr_fbm(h, INTEGER(rowInd), nr, INTEGER(colInd), nc, REAL(sumX), REAL(denoX), INTEGER(ordInd), REAL(pos),
+                                Rf_asReal(size), Rf_asReal(thr), keep);
+  fbm_unmap(keep, bytes, 1);
+  chk(rc);
+  return sqcor;
+}
+
 /* _bigsnpr_readbina2: src/read-plink.cpp:61-80 (5 arguments; BM is the destination FBM.code256, filled in place; the R
  * wrapper creates it with exactly length(ind_row) x length(ind_col) bytes, R/read-plink.R:93-100) */
 SEXP _bigsnpr_readbina2(SEXP BM, SEXP obj_bed, SEXP ind_row, SEXP ind_col, SEXP ncores) {
@@ -465,6 +486,7 @@ static const R_CallMethodDef CallEntries[] = {
     {"_bigsnpr_ld_scores", (DL_FUNC)&_bigsnpr_ld_scores, 6},
     {"_bigsnpr_bed_clumping_chr", (DL_FUNC)&_bigsnpr_bed_clumping_chr, 12},
     {"_bigsnpr_clumping_chr", (DL_FUNC)&_bigsnpr_clumping_chr, 12},
+    {"_bigsnpr_clumping_chr_cached", (DL_FUNC)&_bigsnpr_clumping_chr_cached, 14},
     {"_bigsnpr_readbina2", (DL_FUNC)&_bigsnpr_readbina2, 5},
     {"_bigsnpr_writebina", (DL_FUNC)&_bigsnpr_writebina, 5},
     {"_bigsnpr_prod_and_rowSumsSq", (DL_FUNC)&_bigsnpr_prod_and_rowSumsSq, 6},
