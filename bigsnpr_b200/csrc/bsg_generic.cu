@@ -50,8 +50,8 @@ template <int KIND>
 __global__ void k_pairs(const uint8_t *__restrict__ raw, int64_t n_tot, const double *__restrict__ code3,
                         const double *__restrict__ code, const int *__restrict__ rows, int nr, const int *__restrict__ cols,
                         int nc, const int *__restrict__ wlen, const long long *__restrict__ boff, long long total,
-                        const double *__restrict__ thr, double *__restrict__ band, uint8_t *__restrict__ keep,
-                        const double *__restrict__ sumX, const double *__restrict__ denoX, double thr_r2) {
+                        const double *__restrict__ thr, int nlev, double *__restrict__ band, uint8_t *__restrict__ keep,
+                        const double *__restrict__ sumX, const double *__restrict__ denoX) {
   const long long warp = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5, nw = ((long long)gridDim.x * blockDim.x) >> 5;
   const int lane = threadIdx.x & 31;
   for (long long o = warp; o < total; o += nw) {
@@ -62,7 +62,7 @@ __global__ void k_pairs(const uint8_t *__restrict__ raw, int64_t n_tot, const do
     }
     const int j0 = lo, j = j0 - 1 - (int)(o - boff[j0]);
     const uint8_t *cx = raw + (int64_t)(cols ? cols[j0] : j0) * n_tot, *cy = raw + (int64_t)(cols ? cols[j] : j) * n_tot;
-    if (KIND == 3 || KIND == 4) {
+    if (KIND == BAND_LEVELS) {
       // xySum with the accessor's values (NA_real for a missing code: the sum and r2 are NA, never > thr)
       double xy = 0;
       for (int i = lane; i < nr; i += 32) {
@@ -73,13 +73,9 @@ __global__ void k_pairs(const uint8_t *__restrict__ raw, int64_t n_tot, const do
       if (lane == 0) {
         const double num = xy - sumX[j] * sumX[j0] / nr;
         const double r2 = num * num / (denoX[j] * denoX[j0]);
-        if (KIND == 3) {
-          keep[o] = (r2 > thr_r2) ? 1 : 0;  // false for NaN
-        } else {  // level: how many of the (int)thr_r2 sorted thresholds thr[] r2 exceeds
-          int l = 0;
-          for (int t = 0; t < (int)thr_r2; t++) l += r2 > thr[t];
-          keep[o] = (uint8_t)l;
-        }
+        int l = 0;  // how many of the nlev sorted thresholds thr[] r2 exceeds
+        for (int t = 0; t < nlev; t++) l += r2 > thr[t];
+        keep[o] = (uint8_t)l;
       }
       continue;
     }
@@ -168,19 +164,12 @@ int generic_colstats(bsg_bed *h, const int *d_row, int nr, const int *d_col, int
 }
 
 int generic_pairs(bsg_bed *h, const int *d_row, int nr, const int *d_col, int nc, int kind, const int *d_wlen,
-                  const long long *d_boff, long long total, const double *d_thr, double *d_band, uint8_t *d_keep,
-                  const double *d_sumX, const double *d_denoX, double thr_r2, cudaStream_t s) {
+                  const long long *d_boff, long long total, const double *d_thr, int nlev, double *d_band, uint8_t *d_keep,
+                  const double *d_sumX, const double *d_denoX, cudaStream_t s) {
   if (total <= 0) return BSG_OK;
-  const int grid = gen::grid_warps(total);
-  const double *c3 = h->d_code + 256;
-  if (kind == 0)
-    gen::k_pairs<0><<<grid, 256, 0, s>>>(h->raw, h->n, c3, h->d_code, d_row, nr, d_col, nc, d_wlen, d_boff, total, d_thr, d_band, d_keep, d_sumX, d_denoX, thr_r2);
-  else if (kind == 1)
-    gen::k_pairs<1><<<grid, 256, 0, s>>>(h->raw, h->n, c3, h->d_code, d_row, nr, d_col, nc, d_wlen, d_boff, total, d_thr, d_band, d_keep, d_sumX, d_denoX, thr_r2);
-  else if (kind == 4)
-    gen::k_pairs<4><<<grid, 256, 0, s>>>(h->raw, h->n, c3, h->d_code, d_row, nr, d_col, nc, d_wlen, d_boff, total, d_thr, d_band, d_keep, d_sumX, d_denoX, thr_r2);
-  else
-    gen::k_pairs<3><<<grid, 256, 0, s>>>(h->raw, h->n, c3, h->d_code, d_row, nr, d_col, nc, d_wlen, d_boff, total, d_thr, d_band, d_keep, d_sumX, d_denoX, thr_r2);
+  const auto k = kind == BAND_COR ? gen::k_pairs<BAND_COR> : kind == BAND_LD ? gen::k_pairs<BAND_LD> : gen::k_pairs<BAND_LEVELS>;
+  k<<<gen::grid_warps(total), 256, 0, s>>>(h->raw, h->n, h->d_code + 256, h->d_code, d_row, nr, d_col, nc, d_wlen, d_boff, total,
+                                           d_thr, nlev, d_band, d_keep, d_sumX, d_denoX);
   count_launch();
   BSG_CUDA(cudaGetLastError());
   return BSG_OK;

@@ -9,8 +9,8 @@
 // Both operands of mma.sync.m16n8k32.u8.u8 come straight from the packed words of their lines: a register of the
 // A fragment and a register of the B fragment are both "4 consecutive-k bytes of one line", i.e. a class mask
 // ((plane >> 2c) & 0x03030303) of the same word index -- no shared-memory staging, no per-element unpack.
-// Used by the windowed correlations (bsg_cor.cu) and, with a per-k weight digit folded into the B bytes, by the
-// Gram product of bed_tcrossprodSelf (bsg_la.cu).  The wgmma helpers at the end serve the 128 x 128 tile kernels.
+// Used, with a per-k weight digit folded into the B bytes, by the Gram product of bed_tcrossprodSelf (bsg_la.cu).  The
+// wgmma helpers at the end serve the 128 x 128 tile kernels, which the windowed correlations (bsg_cor.cu) run on.
 #pragma once
 #include <stdint.h>
 
@@ -27,7 +27,7 @@ enum Plane { PL_A = 0, PL_B = 1, PL_H = 2 };
 struct Tile {
   int i0, j0;        // first A line, first B line
   int mode;          // 0: one product (a,a), codes without missing values; 1: the six products of the NA-aware cor
-  long long out;     // offset (in int32) of this tile's sums: [nprod][TM][TN]
+  long long out;     // offset (in int32) of this tile's sums: [nprod][TM][128]
 };
 
 __device__ __forceinline__ void mma_u8u8(int (&d)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0,

@@ -166,7 +166,8 @@ int bsg_ld_scores(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, in
 void bsg_free(void *ptr);
 /* bed_clumping_chr: src/clumping-bed.cpp:11-91.  ordInd = 1-based positions (within ind_col) by decreasing
  * priority; center / scale / pos per selected column; keep[nc] receives 0 / 1.  Pair statistics come from the same
- * Gram tiles as bsg_cor; the greedy sweep in rank order (the sequential part of the algorithm) runs on the host. */
+ * Gram tiles as bsg_cor; the greedy sweep in rank order is resolved on the device in rounds.  An ordInd that is not a
+ * permutation of 1..nc (an entry out of range or repeated): BSG_ERR_BOUNDS. */
 int bsg_clumping_chr(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, int nc, const double *center,
                      const double *scale, const int *ordInd, const double *pos, double size, double thr,
                      int *keep);

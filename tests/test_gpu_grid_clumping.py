@@ -197,6 +197,8 @@ def test_edge_cases(B, ex):
     assert keep[0] == 1 and set(keep[1:].tolist()) <= {0, 1}
     ref = B.clumping_chr(g, ir, ic, ordv, None, p, st["sumX"], st["denoX"], 5e5, 0.2)
     assert np.array_equal(keep[1:], ref)
+    # a NaN threshold keeps every variant (r2 > NaN is false)
+    assert np.all(B.clumping_chr(g, ir, ic, ordv, None, p, st["sumX"], st["denoX"], 5e5, np.nan) == 1)
     # nc = 0, and no grid point: nothing to do
     e = np.zeros(0, dtype=np.int32)
     _call_grid(B, g, ir, e, np.zeros(0), np.zeros(0), np.zeros(0), [([], [])], [0.2], [5e5])
@@ -207,6 +209,17 @@ def test_edge_cases(B, ex):
         _call_grid(B, g, ir, ic, p, st["sumX"], st["denoX"], [([3, 2], [1, 2])], [0.2], [5e5])
     with pytest.raises(BsgError, match="not sorted"):
         _call_grid(B, g, ir, ic, p[::-1].copy(), st["sumX"], st["denoX"], [([1], [1])], [0.2], [5e5])
+    # the priority order must list every position once: a repeated entry is out of bounds in all three entry points
+    dup = ordv.copy()
+    dup[1] = dup[0]
+    with pytest.raises(BsgError, match="out of bounds"):
+        _call_grid(B, g, ir, ic, p, st["sumX"], st["denoX"], [(ic, dup)], [0.2], [5e5])
+    with pytest.raises(BsgError, match="out of bounds"):
+        B.clumping_chr(g, ir, ic, dup, None, p, st["sumX"], st["denoX"], 5e5, 0.2)
+    gb = B.Bed(os.path.join(GOLDEN, "example.bed"))
+    with pytest.raises(BsgError, match="out of bounds"):
+        B.bed_clumping_chr(gb, gb.rows_along(), ic, np.zeros(300), np.ones(300), dup, None, p, 5e5, 0.2)
+    gb.close()
 
 
 def test_shim_clumping_chr_cached(B, oracle, ex, tmp_path_factory):

@@ -6,4 +6,4 @@ n, m, size = int(os.environ.get("N", 100000)), int(os.environ.get("M", 20000)), 
 g = B.Bed.synthetic(n, m, seed=20250927, na_rate=float(os.environ.get("NA", "0")), layouts=B.LAYOUT_SNP_MAJOR)
 for _ in range(2):
     torch.cuda.synchronize(); t = time.perf_counter(); ld = B.bed_ld_scores(g, size=size); torch.cuda.synchronize(); t_ld = time.perf_counter() - t
-print(json.dumps({"gram5": os.environ.get("BSG_GRAM5", "1"), "na": os.environ.get("NA", "0"), "ld_seconds": t_ld, "ld_sum": float(ld.sum())}))
+print(json.dumps({"na": os.environ.get("NA", "0"), "ld_seconds": t_ld, "ld_sum": float(ld.sum())}))
