@@ -61,6 +61,13 @@ SIGNATURES = {
                                    C.c_double, c_int_p]),
     "bsg_grid_clumping_chr": (C.c_int, [vp, c_int_p, C.c_int, c_int_p, C.c_int, c_dbl_p, c_dbl_p, c_dbl_p, C.c_int, c_int_p,
                                         c_int_p, c_int_p, C.c_int, c_dbl_p, c_dbl_p, c_int_p]),
+    "bsg_sfbm_open": (C.c_int, [C.c_int, C.c_int, c_dbl_p, c_dbl_p, c_int_p, C.c_int, C.POINTER(vp)]),
+    "bsg_sfbm_close": (None, [vp]),
+    "bsg_sfbm_nrow": (C.c_int, [vp]),
+    "bsg_sfbm_ncol": (C.c_int, [vp]),
+    "bsg_sfbm_ld_scores": (C.c_int, [vp, c_int_p, C.c_int, c_dbl_p]),
+    "bsg_lassosum2": (C.c_int, [vp, c_dbl_p, C.c_int, c_int_p, C.c_int, c_dbl_p, c_dbl_p, C.c_double, C.c_int, C.c_double,
+                                c_dbl_p, c_int_p, c_dbl_p]),
     "bsg_readbina2": (C.c_int, [vp, c_int_p, C.c_int, c_int_p, C.c_int, C.POINTER(C.c_uint8)]),
     "bsg_writebina": (C.c_int, [vp, C.c_char_p, c_int_p, C.c_int, c_int_p, C.c_int]),
     "bsg_set_prodvec_path": (C.c_int, [C.c_int]),

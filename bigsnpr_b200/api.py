@@ -17,6 +17,7 @@ and error behaviour, so the parity tests read like the reference's testthat file
     prod_and_rowSumsSq / bed_projectSelfPCA   src/bed-fun.cpp:103-133, R/bed-projectPCA.R:45-58,196-227
     multLinReg / bed_pcadapt / snp_pcadapt    src/multLinReg.cpp:8-88, R/pcadapt.R:3-27,61-81
     readbina2 / snp_readBed2, writebina / snp_writeBed   src/read-plink.cpp:61-80, src/write-plink.cpp:13-52
+    as_SFBM / ld_scores_sfbm / snp_lassosum2   bigsparser's SFBM storage, src/ld-scores-sfbm.cpp:9-69, R/lassosum2.R:25-81
 
 Everything computes on the GPU through libbsgpu; there is no CPU path here.
 """
@@ -1130,3 +1131,223 @@ def bed_clumping(obj_bed, ind_row=..., S=None, thr_r2=0.2, size=None, exclude=No
             raise RuntimeError("clumping left undecided variants")
         kept.append(ind_chr[keep == 1])
     return np.sort(np.concatenate(kept)) if kept else np.zeros(0, dtype=np.int32)
+
+
+# ---- sparse LD matrix (bigsparser's SFBM) and lassosum2 -------------------------------------------------------------------
+
+def _full_columns(n, p, i, x, upper):
+    """CSC (p, i, x) of an n x n matrix -> the full symmetric CSC (rows ascending per column), stored entries kept as they
+    are (explicit zeros included).  upper: (p, i, x) holds the upper triangle with the diagonal, mirrored here."""
+    import scipy.sparse as sp
+
+    # canonical order: rows ascending within each column, repeated (row, column) entries summed
+    a = sp.csc_matrix((np.array(x, dtype=np.float64), np.array(i, dtype=np.int64), np.array(p, dtype=np.int64)),
+                      shape=(n, n))  # copies: the caller's arrays stay as they are
+    a.sum_duplicates()
+    p, i, x = a.indptr.astype(np.int64), a.indices.astype(np.int64), a.data
+    if not upper:
+        return p, i, x
+    cnt = np.diff(p)
+    col = np.repeat(np.arange(n, dtype=np.int64), cnt)
+    if np.any(i > col):
+        raise ValueError("'corr' is flagged upper-triangular but stores entries below the diagonal.")
+    # the transpose holds, per column j, the rows >= j in ascending order: its diagonal entry (if any) comes first
+    lt = sp.csc_matrix((x, i, p), shape=(n, n)).T.tocsc()
+    lt.has_sorted_indices = False
+    lt.sort_indices()
+    lp, li, lx = lt.indptr.astype(np.int64), lt.indices.astype(np.int64), lt.data
+    has_diag = np.zeros(n, dtype=bool)
+    nz = cnt > 0
+    has_diag[nz] = i[p[1:][nz] - 1] == np.arange(n)[nz]
+    cnt_l = np.diff(lp) - has_diag
+    fp = np.zeros(n + 1, dtype=np.int64)
+    np.cumsum(cnt + cnt_l, out=fp[1:])
+    fi, fx = np.empty(fp[-1], dtype=np.int64), np.empty(fp[-1])
+    dest = fp[col] + (np.arange(p[-1], dtype=np.int64) - p[col])  # the upper part (with the diagonal) first
+    fi[dest], fx[dest] = i, x
+    lcol = np.repeat(np.arange(n, dtype=np.int64), np.diff(lp))
+    k = np.arange(lp[-1], dtype=np.int64) - lp[lcol]
+    strict = li > lcol
+    dest = fp[lcol] + cnt[lcol] + k - has_diag[lcol]  # then the rows below the diagonal
+    fi[dest[strict]], fx[dest[strict]] = li[strict], lx[strict]
+    return fp, fi, fx
+
+
+def sfbm_storage(corr, compact=False, upper=None):
+    """bigsparser's storage of as_SFBM(corr, compact) as bigsnpr reads it (src/ld-scores-sfbm.cpp:14-66), built on the
+    host: (n, p, data, first_i) with p the ncol + 1 offsets as doubles; non-compact data interleaves (row, value) doubles
+    and first_i is None; compact data holds values only, column j running from its smallest stored row first_i[j] to its
+    largest with zeros filled in (an empty column: first_i 0, no value).
+
+    corr: the (p, i, x) tuple of bed_cor / snp_cor (the upper triangle with the diagonal, expanded to full columns), or a
+    square scipy.sparse matrix, symmetric as stored unless `upper=True` flags an upper-triangular one."""
+    if isinstance(corr, tuple):
+        p, i, x = corr
+        n = len(p) - 1
+        upper = True if upper is None else upper
+    else:
+        import scipy.sparse as sp
+
+        if not sp.issparse(corr):
+            raise TypeError("'corr' must be the (p, i, x) tuple of bed_cor or a scipy.sparse matrix.")
+        if corr.shape[0] != corr.shape[1]:
+            raise ValueError(ERROR_DIM)
+        a = sp.csc_matrix(corr, dtype=np.float64, copy=True)
+        a.sum_duplicates()
+        n, p, i, x = a.shape[0], a.indptr, a.indices, a.data
+        upper = bool(upper)
+    p, i, x = _full_columns(n, p, i, x, upper)
+    if not compact:
+        data = np.empty(2 * x.size)
+        data[0::2], data[1::2] = i, x
+        return n, p.astype(np.float64), data, None
+    cnt = np.diff(p)
+    nz = cnt > 0
+    first_i = np.zeros(n, dtype=np.int32)
+    lens = np.zeros(n, dtype=np.int64)
+    first_i[nz] = i[p[:-1][nz]]
+    lens[nz] = i[p[1:][nz] - 1] - first_i[nz] + 1
+    cp = np.zeros(n + 1, dtype=np.int64)
+    np.cumsum(lens, out=cp[1:])
+    data = np.zeros(cp[-1])
+    col = np.repeat(np.arange(n, dtype=np.int64), cnt)
+    data[cp[col] + (i - first_i[col])] = x
+    return n, cp.astype(np.float64), data, first_i
+
+
+class SFBM:
+    """as_SFBM(corr, compact) on the device (bsg_sfbm_open): the sparse LD matrix snp_lassosum2 and ld_scores_sfbm read.
+    Keeps the host storage arrays `p`, `data` and `first_i` (None when not compact), as the R object exposes them."""
+
+    def __init__(self, nrow, ncol, p, data, first_i=None, device=0):
+        self.p, self.data = _f64(p), _f64(data)
+        self.first_i = None if first_i is None else _i32(first_i)
+        self.compact = first_i is not None
+        h = _lib.vp()
+        check(lib().bsg_sfbm_open(int(nrow), int(ncol), _pd(self.p), _pd(self.data), _pi(self.first_i), int(device),
+                                  C.byref(h)))
+        self._h = h
+
+    @property
+    def nrow(self):
+        return lib().bsg_sfbm_nrow(self._h)
+
+    @property
+    def ncol(self):
+        return lib().bsg_sfbm_ncol(self._h)
+
+    @property
+    def shape(self):
+        return (self.nrow, self.ncol)
+
+    def cols_along(self):
+        return np.arange(1, self.ncol + 1, dtype=np.int32)
+
+    def close(self):
+        if getattr(self, "_h", None):
+            lib().bsg_sfbm_close(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:  # interpreter shutdown
+            pass
+
+
+def as_SFBM(corr, compact=False, upper=None, device=0):
+    """bigsparser::as_SFBM: the sparse LD matrix resident on the device.  corr: the (p, i, x) tuple of bed_cor / snp_cor, or
+    a scipy.sparse matrix (symmetric, or upper-triangular flagged with upper=True).  See sfbm_storage."""
+    n, p, data, first_i = sfbm_storage(corr, compact, upper)
+    return SFBM(n, n, p, data, first_i, device)
+
+
+def ld_scores_sfbm(corr, ind_corr=None, ncores=1):
+    """src/ld-scores-sfbm.cpp:9-69: per column ind_corr[j] (1-based like the rest of this module; default all), the sum of
+    the squared stored values whose row is in ind_corr.  The .Call target receives ind_corr - 1, as here."""
+    ind_sub = np.arange(corr.ncol, dtype=np.int32) if ind_corr is None else _i32(np.asarray(ind_corr) - 1)
+    out = np.empty(ind_sub.size)
+    check(lib().bsg_sfbm_ld_scores(corr._h, _pi(ind_sub), ind_sub.size, _pd(out)))
+    return out
+
+
+def seq_log(from_, to, length_out):
+    """R/SCT.R:167-171: exp(seq(log(from), log(to), length.out)), with seq's rule for the points (both ends exact, the
+    inner ones from + i * by) and the C library's exp."""
+    import math
+
+    n = int(length_out)
+    a, b = math.log(from_), math.log(to)
+    if n <= 2:
+        s = np.array([a, b][:n])
+    elif a == b:
+        s = np.full(n, a)
+    else:
+        s = np.concatenate([[a], a + np.arange(1, n - 1) * ((b - a) / (n - 1)), [b]])
+    return np.array([math.exp(v) for v in s])
+
+
+class Lassosum2Grid(np.ndarray):
+    """snp_lassosum2's result: the m x ngrid matrix of effects with the `grid_param` attribute (dict of columns lambda,
+    delta, num_iter, time, sparsity, one row per column of the matrix)."""
+
+    grid_param = None
+
+
+def _df_column(df, name):
+    try:
+        if name in df:
+            return _f64(df[name])
+    except TypeError:
+        pass
+    raise ValueError("'df_beta' should have element '%s'." % name)
+
+
+def _lassosum2_grid(beta, beta_se, n_eff, delta, nlambda, lambda_min_ratio):
+    """R/lassosum2.R:40-51 and the arguments of every lassosum2 call (:58-67): (beta_hat, scale, lambda and delta of each
+    grid point in expand.grid order, lambda fastest, then the m x ngrid lambda and delta_plus_one matrices)."""
+    N = n_eff
+    scale = np.sqrt(N * beta_se ** 2 + beta ** 2)
+    beta_hat = beta / scale
+    pf = np.sqrt(np.max(N) / N)
+    lambda0 = np.max(np.abs(beta_hat / pf))
+    seq_lam = seq_log(lambda0, lambda_min_ratio * lambda0, nlambda + 1)[1:]
+    g_lam, g_delta = np.tile(seq_lam, delta.size), np.repeat(delta, seq_lam.size)
+    lam = np.asfortranarray(pf[:, None] * g_lam[None, :])
+    dp1 = np.asfortranarray(pf[:, None] * g_delta[None, :] + 1)
+    return beta_hat, scale, g_lam, g_delta, lam, dp1
+
+
+def snp_lassosum2(corr, df_beta, delta=(0.001, 0.01, 0.1, 1), nlambda=30, lambda_min_ratio=0.01, dfmax=200e3, maxiter=1000,
+                  tol=1e-5, ind_corr=None, ncores=1):
+    """R/lassosum2.R:25-81.  corr: an SFBM (as_SFBM); df_beta: a mapping (dict, data frame) with beta, beta_se and n_eff;
+    ind_corr: 1-based columns of corr, one per row of df_beta.  The whole expand.grid(lambda, delta) grid (lambda fastest)
+    runs in one bsg_lassosum2 call, one device CTA per point.  Returns the m x ngrid effects times `scale`, with
+    `grid_param`."""
+    if not hasattr(df_beta, "__getitem__") or not hasattr(df_beta, "__contains__"):
+        raise TypeError("'df_beta' is not of class 'data.frame'.")
+    beta, beta_se, n_eff = (_df_column(df_beta, k) for k in ("beta", "beta_se", "n_eff"))
+    if not isinstance(corr, SFBM):
+        raise TypeError("'corr' is not of class 'SFBM'.")
+    ind_corr = corr.cols_along() if ind_corr is None else _i32(ind_corr)
+    _assert_lengths(ind_corr, beta)
+    if np.any((ind_corr < 1) | (ind_corr > corr.ncol)):
+        raise ValueError("all(ind.corr %in% cols_along(corr)) is not TRUE")
+    if not np.all(beta_se > 0):
+        raise ValueError("'df_beta$beta_se' should have only positive values.")
+    delta = _f64(np.asarray(delta, dtype=np.float64).reshape(-1))
+    if not np.all(delta > 0):
+        raise ValueError("'delta' should have only positive values.")
+    beta_hat, scale, g_lam, g_delta, lam, dp1 = _lassosum2_grid(beta, beta_se, n_eff, delta, nlambda, lambda_min_ratio)
+    m, ngrid = beta.size, g_lam.size
+    beta_est = np.empty((m, ngrid), order="F")
+    num_iter = np.empty(ngrid, dtype=np.int32)
+    secs = np.empty(ngrid)
+    ind_sub = _i32(ind_corr - 1)
+    check(lib().bsg_lassosum2(corr._h, _pd(_f64(beta_hat)), m, _pi(ind_sub), ngrid, _pd(lam), _pd(dp1), float(dfmax),
+                              int(maxiter), float(tol), _pd(beta_est), _pi(num_iter), _pd(secs)))
+    sparsity = np.where(np.isnan(beta_est).any(axis=0), np.nan, (beta_est == 0).mean(axis=0))  # colMeans(beta == 0)
+    with np.errstate(invalid="ignore"):  # a diverged point's NA column times scale
+        out = np.asfortranarray(beta_est * scale[:, None]).view(Lassosum2Grid)
+    out.grid_param = {"lambda": g_lam, "delta": g_delta, "num_iter": num_iter, "time": secs, "sparsity": sparsity}
+    return out

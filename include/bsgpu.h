@@ -230,6 +230,33 @@ int bsg_grid_clumping_chr(bsg_bed *h, const int *ind_row, int nr, const int *ind
                           const double *sumX, const double *denoX, int nsub, const int *sub_len, const int *sub_col,
                           const int *sub_ord, int npt, const double *thr_r2, const double *size_bp, int *keep);
 
+/* ---- sparse LD matrix (bigsparser's SFBM) and summary-statistics PRS -------------------------------------- */
+/* as_SFBM(corr[, compact]) staged to HBM once, in bigsparser's storage as bigsnpr reads it (src/ld-scores-sfbm.cpp:14-66):
+ *   - p: ncol + 1 doubles, non-decreasing integers starting at 0 (X$p);
+ *   - first_i == NULL (non-compact): data interleaves (row, value) doubles, column j at data[2 p[j] .. 2 p[j + 1]), rows
+ *     0-based integers in [0, nrow), each at most once per column;
+ *   - first_i != NULL (compact): data holds values only, column j at data[p[j] .. p[j + 1]) for the contiguous rows
+ *     first_i[j], first_i[j] + 1, ..., which must stay below nrow.
+ * Columns hold the full symmetric matrix (both triangles and the diagonal).  The device keeps either form as given: int32
+ * rows or first_i, fp64 values.  Malformed storage: BSG_ERR_ARG; not enough device memory: BSG_ERR_ALLOC. */
+typedef struct bsg_sfbm bsg_sfbm;
+int bsg_sfbm_open(int nrow, int ncol, const double *p, const double *data, const int *first_i, int device, bsg_sfbm **out);
+void bsg_sfbm_close(bsg_sfbm *s);
+int bsg_sfbm_nrow(const bsg_sfbm *s);
+int bsg_sfbm_ncol(const bsg_sfbm *s);
+/* ld_scores_sfbm: src/ld-scores-sfbm.cpp:9-69.  ind_sub: m 0-based columns (as the .Call target receives them); out[j] =
+ * sum of x^2 over the stored entries of column ind_sub[j] whose row is in ind_sub.  ind_sub out of range: BSG_ERR_BOUNDS. */
+int bsg_sfbm_ld_scores(bsg_sfbm *s, const int *ind_sub, int m, double *out);
+/* lassosum2: src/lassosum2.cpp:20-70 for ngrid grid points in one launch (one CTA per point, every sweep in the kernel).
+ * lambda and delta_plus_one are m x ngrid column-major: column g is what R/lassosum2.R:58-67 passes for ic = g.
+ * beta_est (m x ngrid) and num_iter[ngrid] are bit-identical to the sequential loop; a diverged point (gap > gap0) gets
+ * NA_real in its whole column; num_iter is maxiter + 1 when maxiter sweeps did not stop it.  seconds[ngrid] (NULL
+ * allowed): device time of each point.  ind_sub: m 0-based columns, any order, repeats allowed (BSG_ERR_BOUNDS out of
+ * range); the matrix must be square (BSG_ERR_DIM). */
+int bsg_lassosum2(bsg_sfbm *corr, const double *beta_hat, int m, const int *ind_sub, int ngrid, const double *lambda,
+                  const double *delta_plus_one, double dfmax, int maxiter, double tol, double *beta_est, int *num_iter,
+                  double *seconds);
+
 /* ---- Gram product --------------------------------------------------------------------------------- */
 /* bed_tcrossprodSelf's block loop collapsed into one call: R/bed-tcrossprodSelf.R:38-49 +
  * src/bed-mat-acc.cpp:30-49.  K is nr x nr; center/scale are the per-column scaling (length nc). */

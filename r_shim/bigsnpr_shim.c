@@ -470,6 +470,86 @@ SEXP _bigsnpr_group_tcrossprod_gpu(SEXP grp, SEXP ind_row, SEXP ind_col, SEXP ce
   return K;
 }
 
+/* ---- sparse LD matrix (bigsparser's SFBM) ----------------------------------------------------------------------------
+ * An SFBM environment carries $p (ncol + 1 doubles), $nrow, $ncol and, in the compact form, $first_i (ncol integers); the
+ * reference reads $p and $first_i the same way (src/ld-scores-sfbm.cpp:18,29).  The stored doubles live in a data file:
+ * interleaved (row, value) pairs, 2 p[ncol] doubles, or p[ncol] values when compact.  The field naming that file is taken
+ * to be $sbk; bigsparser is not vendored, so this name is unconfirmed until the shim runs under R (INTEGRATION.md).  The
+ * file is mapped once, staged to HBM, and the handle is cached in the environment (variable ".bsg_sfbm"). */
+static void sfbm_finalizer(SEXP xp) {
+  bsg_sfbm *s = (bsg_sfbm *)R_ExternalPtrAddr(xp);
+  if (s) bsg_sfbm_close(s);
+  R_ClearExternalPtr(xp);
+}
+static bsg_sfbm *sfbm_handle_of(SEXP obj) {
+  SEXP cached = Rf_findVarInFrame(obj, Rf_install(".bsg_sfbm"));
+  if (cached != R_UnboundValue && TYPEOF(cached) == EXTPTRSXP && R_ExternalPtrAddr(cached))
+    return (bsg_sfbm *)R_ExternalPtrAddr(cached);
+  int nrow = Rf_asInteger(field(obj, "nrow")), ncol = Rf_asInteger(field(obj, "ncol"));
+  SEXP p = PROTECT(Rf_coerceVector(field(obj, "p"), REALSXP));
+  if (ncol < 0 || LENGTH(p) != ncol + 1) Rf_error("Incompatibility between dimensions.");
+  SEXP fi = has_field(obj, "first_i") ? field(obj, "first_i") : R_NilValue;
+  const int compact = fi != R_NilValue && LENGTH(fi) == ncol && ncol > 0;
+  if (compact) fi = Rf_coerceVector(fi, INTSXP);
+  PROTECT(fi);
+  const double nval = ncol > 0 ? REAL(p)[ncol] : 0;
+  if (!(nval >= 0) || nval > 4e15) Rf_error("Inconsistency between size of backingfile and dimensions.");
+  const size_t want = (size_t)nval * (compact ? 1 : 2) * sizeof(double);
+  SEXP bf = field(obj, "sbk");
+  if (TYPEOF(bf) != STRSXP || LENGTH(bf) < 1) Rf_error("object has no backing file");
+  const char *path = CHAR(STRING_ELT(bf, 0));
+  int fd = open(path, O_RDONLY);
+  if (fd < 0) Rf_error("Error when mapping file:\n  %s.\n", path);
+  struct stat st;
+  if (fstat(fd, &st) != 0 || (size_t)st.st_size < want) {
+    close(fd);
+    Rf_error("Inconsistency between size of backingfile and dimensions.");
+  }
+  void *data = want ? mmap(NULL, want, PROT_READ, MAP_SHARED, fd, 0) : NULL;
+  close(fd);
+  if (want && data == MAP_FAILED) Rf_error("Error when mapping file:\n  %s.\n", path);
+  bsg_sfbm *s = NULL;
+  int rc = bsg_sfbm_open(nrow, ncol, REAL(p), (const double *)data, compact ? INTEGER(fi) : NULL, gpu_device(), &s);
+  if (data) munmap(data, want);
+  chk(rc);
+  SEXP xp = PROTECT(R_MakeExternalPtr(s, R_NilValue, R_NilValue));
+  R_RegisterCFinalizerEx(xp, sfbm_finalizer, TRUE);
+  Rf_defineVar(Rf_install(".bsg_sfbm"), xp, obj);
+  UNPROTECT(3);
+  return s;
+}
+
+/* _bigsnpr_lassosum2: src/lassosum2.cpp:20-70, one grid point per call (R/lassosum2.R:56-69 loops over the grid with
+ * foreach, so each call takes one SM); the batched grid is bsg_lassosum2 with ngrid > 1 (C ABI, Python mirror) */
+SEXP _bigsnpr_lassosum2(SEXP corr, SEXP beta_hat, SEXP lambda, SEXP delta_plus_one, SEXP ind_sub, SEXP dfmax, SEXP maxiter,
+                        SEXP tol) {
+  bsg_sfbm *s = sfbm_handle_of(corr);
+  SEXP bh = PROTECT(Rf_coerceVector(beta_hat, REALSXP)), lam = PROTECT(Rf_coerceVector(lambda, REALSXP));
+  SEXP dp1 = PROTECT(Rf_coerceVector(delta_plus_one, REALSXP)), sub = PROTECT(Rf_coerceVector(ind_sub, INTSXP));
+  int m = LENGTH(bh), it = 0;
+  if (LENGTH(lam) != m || LENGTH(dp1) != m || LENGTH(sub) != m) Rf_error("Incompatibility between dimensions.");
+  SEXP beta = PROTECT(Rf_allocVector(REALSXP, m));
+  chk(bsg_lassosum2(s, REAL(bh), m, INTEGER(sub), 1, REAL(lam), REAL(dp1), Rf_asReal(dfmax), Rf_asInteger(maxiter),
+                    Rf_asReal(tol), REAL(beta), &it, NULL));
+  const char *names[] = {"beta_est", "num_iter", ""};
+  SEXP res = PROTECT(Rf_mkNamed(VECSXP, names));
+  SET_VECTOR_ELT(res, 0, beta);
+  SET_VECTOR_ELT(res, 1, Rf_ScalarInteger(it));
+  UNPROTECT(6);
+  return res;
+}
+
+/* _bigsnpr_ld_scores_sfbm: src/ld-scores-sfbm.cpp:9-69 (ind_sub 0-based, as R/LDpred2.R:228-229 passes it) */
+SEXP _bigsnpr_ld_scores_sfbm(SEXP X, SEXP ind_sub, SEXP ncores) {
+  bsg_sfbm *s = sfbm_handle_of(X);
+  SEXP sub = PROTECT(Rf_coerceVector(ind_sub, INTSXP));
+  int m = LENGTH(sub);
+  SEXP out = PROTECT(Rf_allocVector(REALSXP, m));
+  chk(bsg_sfbm_ld_scores(s, INTEGER(sub), m, REAL(out)));
+  UNPROTECT(2);
+  return out;
+}
+
 /* registration: same table shape as src/RcppExports.cpp:597-640 (only the hot-path rows shown; the other
  * entries of the reference stay as generated) */
 static const R_CallMethodDef CallEntries[] = {
@@ -492,6 +572,8 @@ static const R_CallMethodDef CallEntries[] = {
     {"_bigsnpr_prod_and_rowSumsSq", (DL_FUNC)&_bigsnpr_prod_and_rowSumsSq, 6},
     {"_bigsnpr_prod_and_rowSumsSq2", (DL_FUNC)&_bigsnpr_prod_and_rowSumsSq2, 6},
     {"_bigsnpr_multLinReg", (DL_FUNC)&_bigsnpr_multLinReg, 5},
+    {"_bigsnpr_lassosum2", (DL_FUNC)&_bigsnpr_lassosum2, 8},
+    {"_bigsnpr_ld_scores_sfbm", (DL_FUNC)&_bigsnpr_ld_scores_sfbm, 3},
     {"_bigsnpr_bed_tcrossprod_gpu", (DL_FUNC)&_bigsnpr_bed_tcrossprod_gpu, 5},
     {"_bigsnpr_bed_randomSVD_gpu", (DL_FUNC)&_bigsnpr_bed_randomSVD_gpu, 7},
     {"_bigsnpr_bed_group_gpu", (DL_FUNC)&_bigsnpr_bed_group_gpu, 4},
