@@ -559,10 +559,14 @@ static int launch_cap(int64_t work, int block, int cap) {
 
 static int launch_cap_pub_impl(int64_t work) { return launch_cap(work, 256, 132 * 16); }
 
+// Head-room bits for sums of up to `maxmult` quantised values: with e = 60 - ex - hb every |v 2^e| < 2^(60 - hb), and
+// while 60 - hb >= 53 that double is already an integer, so |rint(v 2^e)| < 2^(60 - hb) and the sum stays below 2^60.
+// From hb = 8 on, rint may round an entry just below the binade up to 2^(60 - hb) itself and 2^hb of them reach 2^60:
+// one more bit there keeps every sum below 2^60 (k_corr adds 8 of them in int64).
 static int hb_bits(int maxmult) {
   int b = 0;
   while ((1 << b) < maxmult) b++;
-  return b;
+  return b >= 8 ? b + 1 : b;
 }
 
 // Digits of the k_pmv layout for a vector over the selected columns (dir 0: lines = samples of copy B) or over the
@@ -1532,6 +1536,10 @@ static int run_pmvT(bsg_view *v, const uint8_t *dig_raw, int plane, const uint8_
 // Digit blocks over the selected columns in k_pmvT's step order.  nv = 1: one vector of make_vals(mode, x, p1, p2),
 // 60 bits, its second value into s_dig2 when `two`.  nv = 2: the vectors x and xb (30 bits each, 4 + 4 slices; xb may
 // be null), scalars in sc[0] / sc[1].  k_prep1 also leaves the block partials of C = sum c z (mode 1).
+// Every selected column gets its own digits, so one quantised value per digit block needs no head-room (hb = 0).  The
+// missing-value vector scattered into qna_full by physical SNP is different: duplicates of a column add up there, and
+// k_corr adds 8 such sums in int64, so the exponent leaves hb_bits(column multiplicity) of head-room (|sum| < 2^60, see
+// hb_bits).
 static int prep_T(bsg_view *v, int mode, const double *x, const double *p1, const double *p2, int nv, const double *xb,
                   bool two, cudaStream_t s, long long *qna_full = nullptr, int na_second = 0) {
   using namespace pmv;
@@ -1539,12 +1547,13 @@ static int prep_T(bsg_view *v, int mode, const double *x, const double *p1, cons
   Scal *sc = v->s_scal.as<Scal>();
   const int nc = v->nc;
   const int nsteps = (nc + TLINES - 1) / TLINES;
+  const int hb = qna_full ? hb_bits(v->col_maxmult) : 0;
   BSG_TRY(v->s_dig1.ensure((size_t)std::max(nsteps, 1) * 256));
   if (two) BSG_TRY(v->s_dig2.ensure((size_t)std::max(nsteps, 1) * 256));
   uint8_t *dig1 = v->s_dig1.as<uint8_t>(), *dig2 = two ? v->s_dig2.as<uint8_t>() : nullptr;
   BSG_CUDA(cudaMemsetAsync(sc, 0, nv * sizeof(Scal), s));
-  k_prep1<<<SUMCZ_BLOCKS, 256, 0, s>>>(mode, x, p1, p2, nc, 0, sc);
-  if (xb) k_prep1<<<SUMCZ_BLOCKS, 256, 0, s>>>(mode, xb, p1, p2, nc, 0, sc + 1);
+  k_prep1<<<SUMCZ_BLOCKS, 256, 0, s>>>(mode, x, p1, p2, nc, hb, sc);
+  if (xb) k_prep1<<<SUMCZ_BLOCKS, 256, 0, s>>>(mode, xb, p1, p2, nc, hb, sc + 1);
   const int grid = launch_cap((int64_t)std::max(nsteps, 1) * TLINES, 256, 1184);
   if (nv == 1)
     k_quantT<1><<<grid, 256, 0, s>>>(mode, x, nullptr, p1, p2, nc, nsteps * TLINES, sc, dig1, dig2, v->d_col, qna_full,
@@ -1785,6 +1794,14 @@ static int cached_view(bsg_bed *h, const int *ind_row, int nr, const int *ind_co
     if (hit && !ind_row) hit = h->cv_row.empty();
     if (hit && ind_col) hit = (int)h->cv_col.size() == nc && memcmp(h->cv_col.data(), ind_col, (size_t)nc * sizeof(int)) == 0;
     if (hit && !ind_col) hit = h->cv_col.empty();
+    // an identity scaling takes the unscaled path on a fresh view (bsg_view_create); a view built for a real scaling
+    // must not serve it, or the bits of a product would depend on the previous call (the loop stops at the first
+    // non-identity entry, so real scalings pay one comparison)
+    if (hit && center) {
+      bool ident = true;
+      for (int j = 0; j < nc && ident; j++) ident = center[j] == 0.0 && scale[j] == 1.0;
+      hit = !ident;
+    }
   }
   if (!hit) {
     if (h->cv) bsg_view_destroy(h->cv);

@@ -82,7 +82,8 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap *map
 // half sl (chunk ^ 2 sl), relative to the lane's i = sl = 0
 __host__ __device__ constexpr uint32_t TRD(int i, int sl) { return (uint32_t)((i << 7) ^ (i << 4) ^ (sl << 5)); }
 
-// e = bits - exponent(maxabs) - hb, so that |sum of <= 2^hb quantised values| < 2^bits.  bits = 60: one vector in 8
+// e = bits - exponent(maxabs) - hb, so that |sum of <= 2^hb quantised values| < 2^bits (bits = 60: hb_bits in
+// bsg_pmv.cu adds a bit where rint could round an entry up to 2^(bits - hb)).  bits = 60: one vector in 8
 // signed base-256 digits; bits = 30: one of two vectors sharing a pass in 4 digits (max 127 * (2^32 - 1) / 255).
 __device__ __forceinline__ int pick_e(double m, int hb, int bits) {
   int ex = 0;
