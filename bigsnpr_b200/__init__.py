@@ -11,6 +11,7 @@ from .api import (  # noqa: F401
     snp_pcadapt, bed_autoSVD, snp_autoSVD, clumping_chr, clumping_chr_cached, snp_clumping, snp_grid_clumping, readbina2, snp_readBed2, snp_writeBed, writebina, bed_cor, bed_counts, bed_cprodVec, bed_ld_scores, bed_prodVec, bed_randomSVD, bed_scaleBinom,
     bed_tcrossprodSelf, corMat, cor_thresholds, read_bed, read_bed_scaled, snp_MAF, snp_colstats, snp_cor,
     snp_ld_scores, snp_scaleBinom, code256_dosage_scale, prod_and_rowSumsSq2,
-    snp_projectSelfPCA, SFBM, as_SFBM, ld_scores_sfbm, seq_log, snp_lassosum2)
+    snp_projectSelfPCA, SFBM, as_SFBM, ld_scores_sfbm, seq_log, snp_lassosum2,
+    LDCorr, snp_ldsplit)
 
 __all__ = [n for n in dir() if not n.startswith("_")]

@@ -68,7 +68,16 @@ SIGNATURES = {
     "bsg_sfbm_ld_scores": (C.c_int, [vp, c_int_p, C.c_int, c_dbl_p]),
     "bsg_lassosum2": (C.c_int, [vp, c_dbl_p, C.c_int, c_int_p, C.c_int, c_dbl_p, c_dbl_p, C.c_double, C.c_int, C.c_double,
                                 c_dbl_p, c_int_p, c_dbl_p]),
-    "bsg_readbina2": (C.c_int, [vp, c_int_p, C.c_int, c_int_p, C.c_int, C.POINTER(C.c_uint8)]),
+    "bsg_ldcorr_open": (C.c_int, [C.c_int, c_i64_p, c_int_p, c_dbl_p, C.c_int, C.POINTER(vp)]),
+    "bsg_ldcorr_close": (None, [vp]),
+    "bsg_ldcorr_m": (C.c_int, [vp]),
+    "bsg_ldcorr_sumsq2": (C.c_double, [vp]),
+    "bsg_ldcorr_l_triplets": (C.c_int, [vp, C.c_double, C.c_double, c_i64_p, C.c_int64, c_int_p, c_int_p, c_dbl_p]),
+    "bsg_ldsplit": (C.c_int, [vp, C.c_double, C.c_int, c_int_p, C.c_int, C.c_int, C.c_double, C.c_double, c_dbl_p, c_int_p,
+                              c_dbl_p, c_dbl_p, c_dbl_p, c_int_p, c_int_p, c_dbl_p]),
+    "bsg_ldsplit_costs": (C.c_int, [C.c_int, c_i64_p, c_int_p, c_dbl_p, C.c_int, C.c_int, C.c_int, C.c_double, c_dbl_p, C.c_int,
+                                    c_dbl_p, c_int_p]),
+    "bsg_readbina2":(C.c_int, [vp, c_int_p, C.c_int, c_int_p, C.c_int, C.POINTER(C.c_uint8)]),
     "bsg_writebina": (C.c_int, [vp, C.c_char_p, c_int_p, C.c_int, c_int_p, C.c_int]),
     "bsg_set_prodvec_path": (C.c_int, [C.c_int]),
     "bsg_set_scaling_reuse": (C.c_int, [C.c_int]),

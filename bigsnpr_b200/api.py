@@ -18,6 +18,7 @@ and error behaviour, so the parity tests read like the reference's testthat file
     multLinReg / bed_pcadapt / snp_pcadapt    src/multLinReg.cpp:8-88, R/pcadapt.R:3-27,61-81
     readbina2 / snp_readBed2, writebina / snp_writeBed   src/read-plink.cpp:61-80, src/write-plink.cpp:13-52
     as_SFBM / ld_scores_sfbm / snp_lassosum2   bigsparser's SFBM storage, src/ld-scores-sfbm.cpp:9-69, R/lassosum2.R:25-81
+    snp_ldsplit / get_L / get_C   R/split-LD.R:3-40,99-138, src/split-LD.cpp:15-61,65-145,149-182
 
 Everything computes on the GPU through libbsgpu; there is no CPU path here.
 """
@@ -1351,3 +1352,178 @@ def snp_lassosum2(corr, df_beta, delta=(0.001, 0.01, 0.1, 1), nlambda=30, lambda
         out = np.asfortranarray(beta_est * scale[:, None]).view(Lassosum2Grid)
     out.grid_param = {"lambda": g_lam, "delta": g_delta, "num_iter": num_iter, "time": secs, "sparsity": sparsity}
     return out
+
+
+# ---- near-independent LD blocks (snp_ldsplit) ------------------------------------------------------------------------------
+
+def ldsplit_lower(corr, upper=None):
+    """Matrix::tril(corr) in CSC: (p int64, i int32, x float64), rows ascending within each column, repeated entries summed,
+    explicit zeros kept.  corr: the (p, i, x) upper-triangle tuple of bed_cor / snp_cor (upper defaults to True), or a
+    square scipy.sparse matrix, symmetric as stored unless `upper=True` flags an upper-triangular one (as in as_SFBM)."""
+    import scipy.sparse as sp
+
+    if isinstance(corr, tuple):
+        p, i, x = corr
+        n = len(p) - 1
+        a = sp.csc_matrix((np.array(x, dtype=np.float64), np.array(i, dtype=np.int64), np.array(p, dtype=np.int64)),
+                          shape=(n, n))
+        upper = True if upper is None else upper
+    else:
+        if not sp.issparse(corr):
+            raise TypeError("'corr' must be the (p, i, x) tuple of bed_cor or a scipy.sparse matrix.")
+        if corr.shape[0] != corr.shape[1]:
+            raise ValueError(ERROR_DIM)
+        a = sp.csc_matrix(corr, dtype=np.float64, copy=True)
+        upper = bool(upper)
+    a.sum_duplicates()
+    if upper:
+        col = np.repeat(np.arange(a.shape[0]), np.diff(a.indptr))
+        if np.any(a.indices > col):
+            raise ValueError("'corr' is flagged upper-triangular but stores entries below the diagonal.")
+        a = a.T.tocsc()
+    else:
+        a = sp.tril(a, format="csc")
+    a.has_sorted_indices = False
+    a.sort_indices()
+    return a.indptr.astype(np.int64), a.indices.astype(np.int32), a.data.astype(np.float64)
+
+
+def _ldsplit_args(m, min_size, max_size, max_K, max_cost, pos_scaled):
+    """R/split-LD.R:105-106, plus max_size >= min_size and max_K >= 1: (max_size, pos_scaled, max_cost)."""
+    max_size = np.atleast_1d(np.asarray(max_size))
+    if max_size.size == 0 or not np.all(max_size == np.round(max_size)):
+        raise ValueError("'max_size' must be whole numbers.")
+    if not (min_size >= 1 and np.all(max_size <= m)):
+        raise ValueError("min_size >= 1 && all(max_size <= m) is not TRUE")
+    if np.any(max_size < min_size):
+        raise ValueError("'max_size' must be at least 'min_size'.")
+    if max_K < 1:
+        raise ValueError("'max_K' must be at least 1.")
+    pos = np.zeros(m) if pos_scaled is None else _f64(pos_scaled)
+    _assert_lengths(pos, np.empty(m))
+    return max_size, pos, (m / 200 if max_cost is None else float(max_cost))
+
+
+def _check_diag(p, i, x):
+    m = p.size - 1
+    has = np.diff(p) > 0
+    diag = np.zeros(m, dtype=bool)
+    diag[has] = (i[p[:-1][has]] == np.arange(m)[has]) & (x[p[:-1][has]] != 0)
+    if not np.all(diag):
+        raise ValueError("all(Matrix::diag(corr) != 0) is not TRUE")
+
+
+class LDCorr:
+    """Matrix::tril(corr) resident on the device (bsg_ldcorr_open), the input of snp_ldsplit and get_L.  One handle
+    serves any number of calls."""
+
+    def __init__(self, corr, upper=None, device=0):
+        self.p, self.i, self.x = ldsplit_lower(corr, upper) if not isinstance(corr, LDCorr) else (corr.p, corr.i, corr.x)
+        self.m = self.p.size - 1
+        if self.m < 1:
+            raise ValueError("'corr' has no column.")
+        _check_diag(self.p, self.i, self.x)
+        h = _lib.vp()
+        check(lib().bsg_ldcorr_open(self.m, self.p.ctypes.data_as(_lib.c_i64_p), _pi(self.i), _pd(self.x), int(device),
+                                    C.byref(h)))
+        self._h = h
+
+    @property
+    def sumsq2(self):
+        return lib().bsg_ldcorr_sumsq2(self._h)
+
+    def get_L(self, thr_r2, max_r2):
+        """src/split-LD.cpp:15-61: dict of 0-based i (column of corr), j (row) and x, by column and row descending."""
+        n = C.c_int64(0)
+        check(lib().bsg_ldcorr_l_triplets(self._h, float(thr_r2), float(max_r2), C.byref(n), 0, None, None, None))
+        li, lj, lx = np.empty(n.value, dtype=np.int32), np.empty(n.value, dtype=np.int32), np.empty(n.value)
+        check(lib().bsg_ldcorr_l_triplets(self._h, float(thr_r2), float(max_r2), C.byref(n), n.value, _pi(li), _pi(lj), _pd(lx)))
+        return {"i": li, "j": lj, "x": lx}
+
+    def split(self, thr_r2, min_size, max_size, max_K=500, max_r2=0.3, max_cost=None, pos_scaled=None):
+        """snp_ldsplit on this handle: (table or None, layers run per sorted max_size, device seconds of building E, of
+        the layers and of the paths).  See snp_ldsplit."""
+        m = self.m
+        max_size, pos, max_cost = _ldsplit_args(m, min_size, max_size, max_K, max_cost, pos_scaled)
+        S = _i32(max_size)
+        ns, K = S.size, int(max_K)
+        T = K * (K + 1) // 2
+        kept = np.empty(ns * K, dtype=np.int32)
+        cost, cost2, perc = np.empty(ns * K), np.empty(ns * K), np.empty(ns * K)
+        path = np.empty(ns * T, dtype=np.int32)
+        layers = np.empty(ns, dtype=np.int32)
+        secs = np.empty(3)
+        check(lib().bsg_ldsplit(self._h, float(thr_r2), int(min_size), _pi(S), ns, K, float(max_r2), max_cost, _pd(pos),
+                                _pi(kept), _pd(cost), _pd(cost2), _pd(perc), _pi(path), _pi(layers), _pd(secs)))
+        rows = np.flatnonzero(kept == 1)
+        if rows.size == 0:
+            return None, layers, secs
+        t, nb = rows // K, rows % K + 1
+        all_last = [path[tt * T + k * (k - 1) // 2: tt * T + k * (k + 1) // 2].copy() for tt, k in zip(t, nb)]
+        table = {"max_size": np.sort(S)[t].astype(np.int32), "n_block": nb.astype(np.int32), "cost": cost[rows],
+                 "cost2": cost2[rows], "perc_kept": perc[rows], "all_last": all_last,
+                 "all_size": [np.diff(np.concatenate([[0], a])).astype(np.int32) for a in all_last]}
+        return table, layers, secs
+
+    def close(self):
+        if getattr(self, "_h", None):
+            lib().bsg_ldcorr_close(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:  # interpreter shutdown
+            pass
+
+
+def snp_ldsplit(corr, thr_r2, min_size, max_size, max_K=500, max_r2=0.3, max_cost=None, pos_scaled=None, upper=None):
+    """R/split-LD.R:99-138: split a correlation matrix in near-independent blocks, for every max_size value (any order,
+    run sorted).  corr: the (p, i, x) upper-triangle tuple of bed_cor, a scipy.sparse matrix (upper= as in as_SFBM), or
+    an LDCorr handle.  max_cost defaults to m / 200 and is capped at 2 * sum(x^2) over the lower triangle (a sequential
+    fold: R's BLAS crossprod can differ in the last bit).  The whole grid runs in one bsg_ldsplit call.  Returns None when
+    no split is kept, else a dict of equal-length columns max_size, n_block, cost, cost2, perc_kept, all_last and
+    all_size (the last two lists of int arrays, all_last 1-based)."""
+    if not isinstance(corr, LDCorr):
+        p, i, x = ldsplit_lower(corr, upper)
+        _ldsplit_args(p.size - 1, min_size, max_size, max_K, max_cost, pos_scaled)
+        _check_diag(p, i, x)
+    h = corr if isinstance(corr, LDCorr) else LDCorr(corr, upper)
+    try:
+        return h.split(thr_r2, min_size, max_size, max_K, max_r2, max_cost, pos_scaled)[0]
+    finally:
+        if h is not corr:
+            h.close()
+
+
+def get_L(p, i, x, thr_r2, max_r2):
+    """src/split-LD.cpp:15-61 on the lower triangle in CSC (p, i, x): dict of 0-based i, j and x triplets."""
+    import scipy.sparse as sp
+
+    n = len(p) - 1
+    h = LDCorr(sp.csc_matrix((np.asarray(x, dtype=np.float64), np.asarray(i), np.asarray(p)), shape=(n, n)))
+    try:
+        return h.get_L(thr_r2, max_r2)
+    finally:
+        h.close()
+
+
+def get_C(L, min_size, max_size, max_K, max_cost, pos_scaled, device=0):
+    """src/split-LD.cpp:65-145: L is the m x (m + 1) scipy.sparse matrix built from get_L's triplets.  Returns a dict with
+    C (m x max_K) and best_ind (1-based, NA_INTEGER where unset)."""
+    import scipy.sparse as sp
+
+    a = sp.csc_matrix(L, dtype=np.float64, copy=True)
+    a.sum_duplicates()
+    m = a.shape[0]
+    if a.shape[1] != m + 1:
+        raise ValueError(ERROR_DIM)
+    pos = _f64(pos_scaled)
+    _assert_lengths(pos, np.empty(m))
+    K = int(max_K)
+    Cm = np.empty((m, max(K, 0)), order="F")
+    best = np.empty((m, max(K, 0)), dtype=np.int32, order="F")
+    lp = a.indptr.astype(np.int64)
+    check(lib().bsg_ldsplit_costs(m, lp.ctypes.data_as(_lib.c_i64_p), _pi(_i32(a.indices)), _pd(_f64(a.data)), int(min_size),
+                                  int(max_size), K, float(max_cost), _pd(pos), int(device), _pd(Cm), _pi(best)))
+    return {"C": Cm, "best_ind": best}

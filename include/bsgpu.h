@@ -257,6 +257,37 @@ int bsg_lassosum2(bsg_sfbm *corr, const double *beta_hat, int m, const int *ind_
                   const double *delta_plus_one, double dfmax, int maxiter, double tol, double *beta_est, int *num_iter,
                   double *seconds);
 
+/* ---- near-independent LD blocks (snp_ldsplit, R/split-LD.R:99-138) -------------------------------------------------- */
+/* Matrix::tril(corr) staged to HBM once: m x m lower triangle in CSC, p[m + 1] (non-decreasing, p[0] = 0), rows i
+ * increasing within each column and in [column, m), the diagonal stored first and non-zero (R/split-LD.R:108-109),
+ * values x.  Malformed input or a zero / missing diagonal: BSG_ERR_ARG.  sumsq2: 2 * sum(x^2), folded in storage order
+ * (R computes it with BLAS crossprod, R/split-LD.R:111, which can differ in the last bit). */
+typedef struct bsg_ldcorr bsg_ldcorr;
+int bsg_ldcorr_open(int m, const long long *p, const int *i, const double *x, int device, bsg_ldcorr **out);
+void bsg_ldcorr_close(bsg_ldcorr *c);
+int bsg_ldcorr_m(const bsg_ldcorr *c);
+double bsg_ldcorr_sumsq2(const bsg_ldcorr *c);
+/* get_L: src/split-LD.cpp:15-61.  *count receives the number of triplets; with cap >= *count, li / lj / lx (0-based
+ * column of corr, row, value) are filled in the reference's order (by column, row descending).  cap = 0: count only. */
+int bsg_ldcorr_l_triplets(bsg_ldcorr *c, double thr_r2, double max_r2, long long *count, long long cap, int *li, int *lj,
+                     double *lx);
+/* The whole snp_ldsplit grid in one call: get_L, get_C (src/split-LD.cpp:65-145) for every max_size value in one pass
+ * over E per layer, reconstruct_paths (R/split-LD.R:3-40) and get_perc (src/split-LD.cpp:149-182), bit-identical to
+ * them.  max_size[n_max_size] in any order, repeats allowed; results are laid out by position t in the sorted list:
+ * row t max_K + K - 1 of kept (1 when the row is part of the result), cost, cost2, perc_kept; the path of (t, K) at
+ * all_last + t max_K (max_K + 1) / 2 + K (K - 1) / 2, K 1-based last indices.  max_cost is capped at sumsq2.  layers
+ * (NULL allowed): the layers get_C ran per t; seconds[3] (NULL allowed): device time of building E, of the layers, of
+ * the paths and perc_kept.  min_size < 1, max_size > m or < min_size, max_K < 1, a missing pos_scaled: BSG_ERR_ARG;
+ * E and the layer state larger than the free device memory: BSG_ERR_ALLOC, with the bytes needed. */
+int bsg_ldsplit(bsg_ldcorr *c, double thr_r2, int min_size, const int *max_size, int n_max_size, int max_K, double max_r2,
+                double max_cost, const double *pos_scaled, int *kept, double *cost, double *cost2, double *perc_kept,
+                int *all_last, int *layers, double *seconds);
+/* get_C: src/split-LD.cpp:65-145 from L in CSC (m x (m + 1): lp[m + 2], rows li increasing within each column, lx), as
+ * R passes it.  C (m x max_K doubles) and best_ind (m x max_K, 1-based, NA_integer_ where unset), column-major.  Same
+ * argument checks and BSG_ERR_ALLOC rule as bsg_ldsplit. */
+int bsg_ldsplit_costs(int m, const long long *lp, const int *li, const double *lx, int min_size, int max_size, int max_K,
+                      double max_cost, const double *pos_scaled, int device, double *C, int *best_ind);
+
 /* ---- Gram product --------------------------------------------------------------------------------- */
 /* bed_tcrossprodSelf's block loop collapsed into one call: R/bed-tcrossprodSelf.R:38-49 +
  * src/bed-mat-acc.cpp:30-49.  K is nr x nr; center/scale are the per-column scaling (length nc). */

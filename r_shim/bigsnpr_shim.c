@@ -550,6 +550,71 @@ SEXP _bigsnpr_ld_scores_sfbm(SEXP X, SEXP ind_sub, SEXP ncores) {
   return out;
 }
 
+/* p of a CSC matrix (integer, or double for very large ones, as R/split-LD.R:127 passes it) as 64-bit offsets */
+static long long *csc_offsets(SEXP p) {
+  SEXP pd = PROTECT(Rf_coerceVector(p, REALSXP));
+  R_xlen_t n = XLENGTH(pd);
+  long long *out = (long long *)R_alloc(n ? n : 1, sizeof(long long));
+  for (R_xlen_t k = 0; k < n; k++) out[k] = (long long)REAL(pd)[k];
+  UNPROTECT(1);
+  return out;
+}
+
+/* _bigsnpr_get_L: src/split-LD.cpp:15-61 on Matrix::tril(corr)'s p, i, x (R/split-LD.R:116-117); list of 0-based i, j,
+ * x triplets in the reference's order.  The matrix is staged for this call only. */
+SEXP _bigsnpr_get_L(SEXP p, SEXP i, SEXP x, SEXP thr_r2, SEXP max_r2) {
+  SEXP ii = PROTECT(Rf_coerceVector(i, INTSXP)), xx = PROTECT(Rf_coerceVector(x, REALSXP));
+  long long *pp = csc_offsets(p);
+  int m = (int)XLENGTH(p) - 1;
+  if (m < 1 || pp[m] != XLENGTH(ii) || XLENGTH(xx) != XLENGTH(ii)) Rf_error("Incompatibility between dimensions.");
+  bsg_ldcorr *c = NULL;
+  chk(bsg_ldcorr_open(m, pp, INTEGER(ii), REAL(xx), gpu_device(), &c));
+  long long n = 0;
+  int rc = bsg_ldcorr_l_triplets(c, Rf_asReal(thr_r2), Rf_asReal(max_r2), &n, 0, NULL, NULL, NULL);
+  if (rc) {
+    bsg_ldcorr_close(c);
+    chk(rc);
+  }
+  const char *names[] = {"i", "j", "x", ""};
+  SEXP res = PROTECT(Rf_mkNamed(VECSXP, names));
+  SEXP ri = PROTECT(Rf_allocVector(INTSXP, n)), rj = PROTECT(Rf_allocVector(INTSXP, n)), rx = PROTECT(Rf_allocVector(REALSXP, n));
+  rc = bsg_ldcorr_l_triplets(c, Rf_asReal(thr_r2), Rf_asReal(max_r2), &n, n, INTEGER(ri), INTEGER(rj), REAL(rx));
+  bsg_ldcorr_close(c);
+  chk(rc);
+  SET_VECTOR_ELT(res, 0, ri);
+  SET_VECTOR_ELT(res, 1, rj);
+  SET_VECTOR_ELT(res, 2, rx);
+  UNPROTECT(6);
+  return res;
+}
+
+/* _bigsnpr_get_C: src/split-LD.cpp:65-145 on the m x (m + 1) dgCMatrix L that R/split-LD.R:118-120 builds (its p, i, x
+ * and Dim slots); list of C (m x max_K) and best_ind.  Any other matrix class is refused. */
+SEXP _bigsnpr_get_C(SEXP L, SEXP min_size, SEXP max_size, SEXP max_K, SEXP max_cost, SEXP pos_scaled) {
+  if (!Rf_inherits(L, "dgCMatrix")) Rf_error("'L' must be a dgCMatrix.");
+  SEXP dim = PROTECT(Rf_coerceVector(Rf_getAttrib(L, Rf_install("Dim")), INTSXP));
+  SEXP li = PROTECT(Rf_coerceVector(Rf_getAttrib(L, Rf_install("i")), INTSXP));
+  SEXP lx = PROTECT(Rf_coerceVector(Rf_getAttrib(L, Rf_install("x")), REALSXP));
+  SEXP pos = PROTECT(Rf_coerceVector(pos_scaled, REALSXP));
+  SEXP lpv = Rf_getAttrib(L, Rf_install("p"));
+  if (XLENGTH(dim) != 2) Rf_error("Incompatibility between dimensions.");
+  int m = INTEGER(dim)[0], K = Rf_asInteger(max_K);
+  if (INTEGER(dim)[1] != m + 1 || XLENGTH(lpv) != (R_xlen_t)m + 2 || XLENGTH(pos) != m || XLENGTH(li) != XLENGTH(lx))
+    Rf_error("Incompatibility between dimensions.");
+  long long *lp = csc_offsets(lpv);
+  if (lp[m + 1] != XLENGTH(li)) Rf_error("Incompatibility between dimensions.");
+  if (K < 1) Rf_error("max_K must be at least 1.");
+  const char *names[] = {"C", "best_ind", ""};
+  SEXP res = PROTECT(Rf_mkNamed(VECSXP, names));
+  SEXP C = PROTECT(Rf_allocMatrix(REALSXP, m, K)), best = PROTECT(Rf_allocMatrix(INTSXP, m, K));
+  chk(bsg_ldsplit_costs(m, lp, INTEGER(li), REAL(lx), Rf_asInteger(min_size), Rf_asInteger(max_size), K,
+                        Rf_asReal(max_cost), REAL(pos), gpu_device(), REAL(C), INTEGER(best)));
+  SET_VECTOR_ELT(res, 0, C);
+  SET_VECTOR_ELT(res, 1, best);
+  UNPROTECT(7);
+  return res;
+}
+
 /* registration: same table shape as src/RcppExports.cpp:597-640 (only the hot-path rows shown; the other
  * entries of the reference stay as generated) */
 static const R_CallMethodDef CallEntries[] = {
@@ -574,6 +639,8 @@ static const R_CallMethodDef CallEntries[] = {
     {"_bigsnpr_multLinReg", (DL_FUNC)&_bigsnpr_multLinReg, 5},
     {"_bigsnpr_lassosum2", (DL_FUNC)&_bigsnpr_lassosum2, 8},
     {"_bigsnpr_ld_scores_sfbm", (DL_FUNC)&_bigsnpr_ld_scores_sfbm, 3},
+    {"_bigsnpr_get_L", (DL_FUNC)&_bigsnpr_get_L, 5},
+    {"_bigsnpr_get_C", (DL_FUNC)&_bigsnpr_get_C, 6},
     {"_bigsnpr_bed_tcrossprod_gpu", (DL_FUNC)&_bigsnpr_bed_tcrossprod_gpu, 5},
     {"_bigsnpr_bed_randomSVD_gpu", (DL_FUNC)&_bigsnpr_bed_randomSVD_gpu, 7},
     {"_bigsnpr_bed_group_gpu", (DL_FUNC)&_bigsnpr_bed_group_gpu, 4},
