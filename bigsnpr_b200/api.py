@@ -19,8 +19,11 @@ and error behaviour, so the parity tests read like the reference's testthat file
     readbina2 / snp_readBed2, writebina / snp_writeBed   src/read-plink.cpp:61-80, src/write-plink.cpp:13-52
     as_SFBM / ld_scores_sfbm / snp_lassosum2   bigsparser's SFBM storage, src/ld-scores-sfbm.cpp:9-69, R/lassosum2.R:25-81
     snp_ldsplit / get_L / get_C   R/split-LD.R:3-40,99-138, src/split-LD.cpp:15-61,65-145,149-182
+    sp_solve_sym / snp_ldpred2_inf   bigsparser's conjugate-gradient solve, R/LDpred2.R:27-42
+    snp_ldsc / snp_ldsc2   R/ldsc.R:1-224 (host NumPy; the LD scores of snp_ldsc2 come from ld_scores_sfbm)
 
-Everything computes on the GPU through libbsgpu; there is no CPU path here.
+Everything computes on the GPU through libbsgpu; there is no CPU path here (LD score regression, a few
+weighted least-squares fits on per-variant vectors, runs on the host).
 """
 from __future__ import annotations
 
@@ -1352,6 +1355,179 @@ def snp_lassosum2(corr, df_beta, delta=(0.001, 0.01, 0.1, 1), nlambda=30, lambda
         out = np.asfortranarray(beta_est * scale[:, None]).view(Lassosum2Grid)
     out.grid_param = {"lambda": g_lam, "delta": g_delta, "num_iter": num_iter, "time": secs, "sparsity": sparsity}
     return out
+
+
+# ---- LDpred2-inf (sp_solve_sym) and LD score regression --------------------------------------------------------------------
+
+def _sp_solve(corr, b, add_to_diag, tol, maxiter):
+    """bsg_sfbm_solve: (x, iters, error) of the conjugate-gradient solve of (corr + diag(add_to_diag)) x = b."""
+    if not isinstance(corr, SFBM):
+        raise TypeError("'corr' is not of class 'SFBM'.")
+    b = _f64(np.asarray(b, dtype=np.float64).reshape(-1))
+    d = _f64(np.asarray(add_to_diag, dtype=np.float64).reshape(-1))
+    n = corr.ncol
+    _assert_lengths(b, range(n))
+    if d.size not in (1, n):
+        raise ValueError(ERROR_DIM)
+    maxiter = 10 * n if maxiter is None else int(maxiter)
+    x = np.empty(n)
+    it, err = C.c_int(), C.c_double()
+    check(lib().bsg_sfbm_solve(corr._h, _pd(b), _pd(d), d.size, float(tol), maxiter, _pd(x), C.byref(it), C.byref(err)))
+    return x, it.value, err.value
+
+
+def sp_solve_sym(corr, b, add_to_diag=0, tol=1e-10, maxiter=None):
+    """bigsparser::sp_solve_sym: x solving (corr + diag(add_to_diag)) x = b by the conjugate gradient on the device
+    (bsg_sfbm_solve).  corr: an SFBM; add_to_diag: one value or one per column; maxiter None is 10 * ncol(corr).  A NaN
+    error raises "Solver failed."; an error above tol warns "Estimated error: <error>."."""
+    x, _, err = _sp_solve(corr, b, add_to_diag, tol, maxiter)
+    if np.isnan(err):
+        raise RuntimeError("Solver failed.")
+    if err > tol:
+        import warnings
+
+        warnings.warn("Estimated error: %g." % err)
+    return x
+
+
+def snp_ldpred2_inf(corr, df_beta, h2):
+    """R/LDpred2.R:27-42: effects under the infinitesimal model, x * scale with x solving
+    (corr + diag(ncol / (h2 * N))) x = beta / scale, scale = sqrt(N * beta_se^2 + beta^2), N = n_eff."""
+    if not hasattr(df_beta, "__getitem__") or not hasattr(df_beta, "__contains__"):
+        raise TypeError("'df_beta' is not of class 'data.frame'.")
+    beta, beta_se, n_eff = (_df_column(df_beta, k) for k in ("beta", "beta_se", "n_eff"))
+    if not isinstance(corr, SFBM):
+        raise TypeError("'corr' is not of class 'SFBM'.")
+    _assert_lengths(range(corr.nrow), range(corr.ncol))
+    _assert_lengths(range(corr.ncol), beta)
+    if not np.all(beta_se > 0):
+        raise ValueError("'df_beta$beta_se' should have only positive values.")
+    h2 = np.asarray(h2, dtype=np.float64)
+    if not np.all(h2 > 0):
+        raise ValueError("'h2' should have only positive values.")
+    N = n_eff
+    scale = np.sqrt(N * beta_se ** 2 + beta ** 2)
+    beta_hat = beta / scale
+    beta_inf = sp_solve_sym(corr, beta_hat, add_to_diag=corr.ncol / (h2 * N))
+    return beta_inf * scale
+
+
+def _wlm(x, y, w):
+    """R/ldsc.R:11-22 (stats::lm.wfit(cbind(1, x), y, w)), in its formula order."""
+    wx = w * x
+    W, WX = np.sum(w), np.sum(wx)
+    WY, WXX, WXY = np.dot(w, y), np.dot(wx, x), np.dot(wx, y)
+    alpha = (WXX * WY - WX * WXY) / (W * WXX - WX ** 2)
+    beta = (WXY * W - WX * WY) / (W * WXX - WX ** 2)
+    return alpha, beta, x * beta + alpha
+
+
+def _wlm_no_int(x, y, w):
+    """R/ldsc.R:25-31 (stats::lm.wfit(as.matrix(x), y, w))."""
+    wx = w * x
+    beta = np.dot(wx, y) / np.dot(wx, x)
+    return beta, x * beta
+
+
+def _weights(pred, w_ld):
+    return 1 / (pred ** 2 * w_ld)
+
+
+def snp_ldsc(ld_score, ld_size, chi2, sample_size, blocks=200, intercept=None, chi2_thr1=30, chi2_thr2=np.inf, ncores=1):
+    """R/ldsc.R:70-170, on the host: LD score regression with the two-step estimator.  blocks None: (int, h2); else a number
+    of blocks of consecutive variants or a block label per variant, and the delete-a-block jackknife gives
+    (int, int_se, h2, h2_se).  intercept None estimates it (step 1, variants with chi2 < chi2_thr1)."""
+    chi2 = _f64(chi2) + 1e-8
+    if not np.all(chi2 > 0):
+        raise ValueError("'chi2' should have only positive values.")
+    ld_score = _f64(ld_score)
+    _assert_lengths(chi2, ld_score)
+    ld_size = np.asarray(ld_size)
+    if ld_size.size != 1:
+        raise ValueError("'ld_size' should be of length 1.")
+    if ld_size != np.trunc(ld_size):
+        raise ValueError("'ld_size' should contain only integers.")
+    ld_size = float(ld_size)
+    M = chi2.size
+    sample_size = _f64(np.asarray(sample_size, dtype=np.float64).reshape(-1))
+    if sample_size.size == 1:
+        sample_size = np.repeat(sample_size, M)
+    else:
+        _assert_lengths(sample_size, chi2)
+
+    if blocks is None:
+        if intercept is None:  # step 1
+            ind_sub1 = chi2 < chi2_thr1
+            w_ld = np.maximum(ld_score[ind_sub1], 1)
+            x1 = (ld_score / ld_size * sample_size)[ind_sub1]
+            y1 = chi2[ind_sub1]
+            pred0 = y1
+            for _ in range(100):
+                pred = _wlm(x1, y1, _weights(pred0, w_ld))[2]
+                if np.max(np.abs(pred - pred0)) < 1e-6:
+                    break
+                pred0 = pred
+            step1_int = _wlm(x1, y1, _weights(pred0, w_ld))[0]
+        else:
+            step1_int = float(intercept)
+        # step 2
+        ind_sub2 = chi2 < chi2_thr2
+        w_ld = np.maximum(ld_score[ind_sub2], 1)
+        x = (ld_score / ld_size * sample_size)[ind_sub2]
+        y = chi2[ind_sub2]
+        yp = y - step1_int
+        pred0 = y
+        for _ in range(100):
+            pred = step1_int + _wlm_no_int(x, yp, _weights(pred0, w_ld))[1]
+            if np.max(np.abs(pred - pred0)) < 1e-6:
+                break
+            pred0 = pred
+        step2_h2 = _wlm_no_int(x, yp, _weights(pred0, w_ld))[0]
+        return np.array([step1_int, step2_h2])
+
+    # delete-a-group jackknife (the fits receive chi2 + 1e-8, to which they add 1e-8 again, as the reference's do)
+    blocks = np.asarray(blocks).reshape(-1)
+    if blocks.size == 1:
+        blocks = np.sort(np.resize(np.arange(1, int(blocks[0]) + 1), M))  # sort(rep_len(seq_len(blocks), M))
+    else:
+        _assert_lengths(blocks, chi2)
+    labels = np.unique(blocks)
+    ind_blocks = [np.flatnonzero(blocks == lab) for lab in labels]  # split(seq_along(blocks), blocks)
+    h_blocks = M / np.array([ib.size for ib in ind_blocks], dtype=np.float64)
+    fits = []
+    for ind_rm in [None] + ind_blocks:
+        keep = np.ones(M, dtype=bool)
+        if ind_rm is not None:
+            keep[ind_rm] = False
+        fits.append(snp_ldsc(ld_score[keep], ld_size, chi2[keep], sample_size[keep], None, intercept, chi2_thr1,
+                             chi2_thr2))
+    delete_values = np.array(fits).T
+    estim = delete_values[:, 0]
+    int_pseudo = h_blocks * estim[0] - (h_blocks - 1) * delete_values[0, 1:]
+    h2_pseudo = h_blocks * estim[1] - (h_blocks - 1) * delete_values[1, 1:]
+    int_J = np.sum(int_pseudo / h_blocks)
+    h2_J = np.sum(h2_pseudo / h_blocks)
+    return np.array([int_J, np.sqrt(np.mean((int_pseudo - int_J) ** 2 / (h_blocks - 1))),
+                     h2_J, np.sqrt(np.mean((h2_pseudo - h2_J) ** 2 / (h_blocks - 1)))])
+
+
+def snp_ldsc2(corr, df_beta, blocks=None, intercept=1, ncores=1, ind_beta=None, chi2_thr1=30, chi2_thr2=np.inf):
+    """R/ldsc.R:202-224 on an SFBM: snp_ldsc with the LD scores of ld_scores_sfbm over all columns, ld_size = ncol(corr),
+    chi2 = (beta / beta_se)^2 and sample_size = n_eff.  ind_beta: 1-based columns of corr, one per row of df_beta."""
+    if not hasattr(df_beta, "__getitem__") or not hasattr(df_beta, "__contains__"):
+        raise TypeError("'df_beta' is not of class 'data.frame'.")
+    beta, beta_se, n_eff = (_df_column(df_beta, k) for k in ("beta", "beta_se", "n_eff"))
+    if not isinstance(corr, SFBM):
+        raise TypeError("'corr' is not of class 'SFBM'.")
+    ind_beta = corr.cols_along() if ind_beta is None else _i32(ind_beta)
+    _assert_lengths(ind_beta, beta)
+    if np.any((ind_beta < 1) | (ind_beta > corr.ncol)):
+        raise ValueError("all(ind.beta %in% cols_along(corr)) is not TRUE")
+    if not np.all(beta_se > 0):
+        raise ValueError("'df_beta$beta_se' should have only positive values.")
+    full_ld = ld_scores_sfbm(corr)
+    return snp_ldsc(full_ld[ind_beta - 1], corr.ncol, (beta / beta_se) ** 2, n_eff, blocks=blocks, intercept=intercept,
+                    chi2_thr1=chi2_thr1, chi2_thr2=chi2_thr2)
 
 
 # ---- near-independent LD blocks (snp_ldsplit) ------------------------------------------------------------------------------

@@ -13,6 +13,17 @@
 // the state as it was, so every coordinate sees exactly the state the sequential loop gives it.  The arithmetic is the
 // reference's, uncontracted: u_j in its order, soft_thres with its IEEE division, the update as dadd(d, dmul(x, shift)),
 // gap folded serially in coordinate order, df a count.  Hence bit-identical beta_est and num_iter.
+//
+// sp_solve_sym (bigsparser, called at R/LDpred2.R:38-39): Eigen's ConjugateGradient with the identity preconditioner and
+// x0 = 0, over A + diag(d) with A the SFBM as stored.  Every sum is taken in one fixed order, independent of the launch:
+//   - (A p + d o p)_j: a warp per column, lane l folding the entries q = lo + l, lo + l + 32, ... in ascending q, then the
+//     xor-shuffle tree 16, 8, 4, 2, 1, then dadd(sum, dmul(d_j, p_j));
+//   - a vector dot u.v: chunks of CG_CH = 1024 entries (entries past n are +0), each summed as a pairwise tree (level 1
+//     pairs k and k + 512, then k and k + 256, ... down to k and k + 1), chunk sums folded serially from 0 in chunk order.
+// No FMA contraction (__dadd_rn / __dsub_rn / __dmul_rn / __ddiv_rn).  One iteration is four launches (t = A p + d o p;
+// chunk sums of p.t; alpha, x, r and chunk sums of r.r; the stopping test and p); a done flag in device memory turns the
+// rest of a block of CG_BLOCK enqueued iterations into no-ops, and the host reads it once per block.
+#include <float.h>
 #include <math.h>
 #include <string.h>
 
@@ -30,6 +41,7 @@ struct bsg_sfbm {
   int *first_i = nullptr;  // ncol first rows (compact)
   double *x = nullptr;     // nnz values
   cudaStream_t stream = nullptr;
+  double last_solve_ms = 0;  // ms, device time of the last bsg_sfbm_solve's iterations (CUDA events)
 };
 
 namespace bsg {
@@ -189,6 +201,163 @@ __global__ void k_ld_scores_sfbm(const long long *__restrict__ p, const int *__r
     for (int o = 16; o; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
     if (lane == 0) out[j] = s;
   }
+}
+
+// ---- sp_solve_sym: conjugate gradient ------------------------------------------------------------------------------------
+
+constexpr int CG_CH = 1024;       // entries per chunk of a vector dot
+constexpr int CG_DT = CG_CH / 2;  // threads of a chunk CTA: two entries each
+constexpr int CG_MT = 256;        // threads of a matvec CTA (a warp per column)
+constexpr int CG_BLOCK = 64;      // iterations enqueued between two reads of the done flag
+
+struct CgState {
+  double ab[2];   // absNew of iteration i in ab[i & 1] (read by every CTA of iteration i, written for i + 1)
+  double rhs2;    // b.b
+  double rn2;     // r.r of the last iteration run
+  int done;       // r.r < threshold was reached
+  int iters;      // the iteration that reached it (Eigen does not count it)
+};
+
+// Sum of the chunk's 1024 values in the fixed pairwise tree; a and b are entries k and k + 512 of thread k.  Valid in
+// thread 0.
+__device__ __forceinline__ double cg_chunk_tree(double a, double b, double *sh) {
+  const int k = threadIdx.x;
+  double s = __dadd_rn(a, b);
+  sh[k] = s;
+  __syncthreads();
+  for (int w = CG_DT / 2; w >= 32; w >>= 1) {
+    if (k < w) sh[k] = s = __dadd_rn(s, sh[k + w]);
+    __syncthreads();
+  }
+  if (k < 32)
+    for (int w = 16; w; w >>= 1) s = __dadd_rn(s, __shfl_down_sync(0xffffffffu, s, w));
+  return s;
+}
+
+// The chunk sums folded serially from 0 in chunk order, by warp 0 (every lane holds the result); broadcast through sh.
+__device__ __forceinline__ double cg_fold(const double *__restrict__ part, int nch, double *sh) {
+  if (threadIdx.x < 32) {
+    const int lane = threadIdx.x;
+    double s = 0;
+    for (int base = 0; base < nch; base += 32) {
+      const double v = base + lane < nch ? part[base + lane] : 0;
+      const int cnt = min(32, nch - base);
+      for (int l = 0; l < cnt; l++) s = __dadd_rn(s, __shfl_sync(0xffffffffu, v, l));
+    }
+    if (lane == 0) sh[0] = s;
+  }
+  __syncthreads();
+  const double s = sh[0];
+  __syncthreads();  // sh is reused by the chunk tree
+  return s;
+}
+
+// x = 0, r = p = b, chunk sums of b.b
+__global__ void __launch_bounds__(CG_DT) k_cg_init(const double *__restrict__ b, int n, double *x, double *r, double *p,
+                                                   double *part) {
+  __shared__ double sh[CG_DT];
+  const int i0 = blockIdx.x * CG_CH + threadIdx.x, i1 = i0 + CG_DT;
+  double a = 0, c = 0;
+  if (i0 < n) {
+    const double v = b[i0];
+    x[i0] = 0, r[i0] = v, p[i0] = v;
+    a = __dmul_rn(v, v);
+  }
+  if (i1 < n) {
+    const double v = b[i1];
+    x[i1] = 0, r[i1] = v, p[i1] = v;
+    c = __dmul_rn(v, v);
+  }
+  const double s = cg_chunk_tree(a, c, sh);
+  if (threadIdx.x == 0) part[blockIdx.x] = s;
+}
+
+__global__ void k_cg_init_fold(const double *__restrict__ part, int nch, CgState *st) {
+  __shared__ double sh[1];
+  const double s = cg_fold(part, nch, sh);
+  if (threadIdx.x == 0) {
+    st->rhs2 = s, st->rn2 = s, st->ab[0] = s, st->ab[1] = 0;
+    st->done = 0, st->iters = 0;
+  }
+}
+
+// t_j = dadd(sum_q x_q p[row_q], dmul(d_j, p_j)); d has length 1 (dlen == 1) or n
+__global__ void __launch_bounds__(CG_MT) k_cg_matvec(const long long *__restrict__ cp, const int *__restrict__ rows,
+                                                     const int *__restrict__ first_i, const double *__restrict__ x, int n,
+                                                     const double *__restrict__ d, int dlen, const double *__restrict__ p,
+                                                     double *__restrict__ t, const CgState *st) {
+  if (st->done) return;
+  const int lane = threadIdx.x & 31;
+  const int nw = (gridDim.x * blockDim.x) >> 5;
+  for (int j = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; j < n; j += nw) {
+    const long long lo = cp[j], up = cp[j + 1];
+    double s = 0;
+    if (rows) {
+#pragma unroll 4
+      for (long long q = lo + lane; q < up; q += 32) s = __dadd_rn(s, __dmul_rn(x[q], p[rows[q]]));
+    } else {  // compact: entry lo + k is row first_i[j] + k
+      const double *xc = x + lo, *pc = p + first_i[j];
+      const int len = (int)(up - lo);
+#pragma unroll 4
+      for (int k = lane; k < len; k += 32) s = __dadd_rn(s, __dmul_rn(xc[k], pc[k]));
+    }
+    for (int o = 16; o; o >>= 1) s = __dadd_rn(s, __shfl_xor_sync(0xffffffffu, s, o));
+    if (lane == 0) t[j] = __dadd_rn(s, __dmul_rn(d[dlen == 1 ? 0 : j], p[j]));
+  }
+}
+
+// chunk sums of p.t
+__global__ void __launch_bounds__(CG_DT) k_cg_pt(const double *__restrict__ p, const double *__restrict__ t, int n,
+                                                 double *part, const CgState *st) {
+  __shared__ double sh[CG_DT];
+  if (st->done) return;
+  const int i0 = blockIdx.x * CG_CH + threadIdx.x, i1 = i0 + CG_DT;
+  const double a = i0 < n ? __dmul_rn(p[i0], t[i0]) : 0, c = i1 < n ? __dmul_rn(p[i1], t[i1]) : 0;
+  const double s = cg_chunk_tree(a, c, sh);
+  if (threadIdx.x == 0) part[blockIdx.x] = s;
+}
+
+// alpha = absNew / p.t (every CTA folds the same chunk sums); x += alpha p; r -= alpha t; chunk sums of r.r
+__global__ void __launch_bounds__(CG_DT) k_cg_update(const double *__restrict__ p, const double *__restrict__ t, int n,
+                                                     double *x, double *r, const double *__restrict__ part_pt, int nch,
+                                                     double *part_rr, const CgState *st, int it) {
+  __shared__ double sh[CG_DT];
+  if (st->done) return;
+  const double alpha = __ddiv_rn(st->ab[it & 1], cg_fold(part_pt, nch, sh));
+  double v[2] = {0, 0};
+#pragma unroll
+  for (int h = 0; h < 2; h++) {
+    const int i = blockIdx.x * CG_CH + threadIdx.x + h * CG_DT;
+    if (i < n) {
+      x[i] = __dadd_rn(x[i], __dmul_rn(alpha, p[i]));
+      const double ri = __dsub_rn(r[i], __dmul_rn(alpha, t[i]));
+      r[i] = ri;
+      v[h] = __dmul_rn(ri, ri);
+    }
+  }
+  const double s = cg_chunk_tree(v[0], v[1], sh);
+  if (threadIdx.x == 0) part_rr[blockIdx.x] = s;
+}
+
+// rn2 = r.r; stop when rn2 < threshold; else beta = rn2 / absOld, p = r + beta p
+__global__ void __launch_bounds__(CG_DT) k_cg_direction(const double *__restrict__ r, int n, double *p,
+                                                        const double *__restrict__ part_rr, int nch, double threshold,
+                                                        CgState *st, int it) {
+  __shared__ double sh[1];
+  if (st->done) return;  // set only by CTA 0 of this launch on convergence, when every CTA returns below anyway
+  const double rn2 = cg_fold(part_rr, nch, sh);
+  const bool lead = blockIdx.x == 0 && threadIdx.x == 0;
+  if (rn2 < threshold) {
+    if (lead) st->rn2 = rn2, st->iters = it, st->done = 1;
+    return;
+  }
+  const double beta = __ddiv_rn(rn2, st->ab[it & 1]);
+#pragma unroll
+  for (int h = 0; h < 2; h++) {
+    const int i = blockIdx.x * CG_CH + threadIdx.x + h * CG_DT;
+    if (i < n) p[i] = __dadd_rn(r[i], __dmul_rn(beta, p[i]));
+  }
+  if (lead) st->rn2 = rn2, st->ab[(it + 1) & 1] = rn2;
 }
 
 static int bind(const bsg_sfbm *s) {
@@ -367,5 +536,93 @@ int bsg_lassosum2(bsg_sfbm *corr, const double *beta_hat, int m, const int *ind_
     for (int g = 0; g < ngrid; g++) seconds[g] = ns[g] * 1e-9;
   return BSG_OK;
 }
+
+int bsg_sfbm_solve(bsg_sfbm *A, const double *b, const double *add_to_diag, int diag_len, double tol, int maxiter,
+                   double *x, int *iters, double *error) {
+  if (!A || !b || !add_to_diag || !x || !iters || !error) return fail(BSG_ERR_ARG, "null argument");
+  if (A->nrow != A->ncol) return fail(BSG_ERR_DIM, "Incompatibility between dimensions.");
+  const int n = A->ncol;
+  if (diag_len != 1 && diag_len != n) return fail(BSG_ERR_DIM, "Incompatibility between dimensions.");
+  if (!(tol >= 0)) return fail(BSG_ERR_ARG, "'tol' must be non-negative.");
+  if (maxiter < 0) return fail(BSG_ERR_ARG, "'maxiter' must be non-negative.");
+  A->last_solve_ms = 0;
+  if (n == 0) {  // b.b == 0
+    *iters = 0, *error = 0;
+    return BSG_OK;
+  }
+  BSG_TRY(bind(A));
+  cudaStream_t st = A->stream;
+  const int nch = (n + CG_CH - 1) / CG_CH;
+  Bufs bf;
+  double *d_b = nullptr, *d_d = nullptr, *d_x = nullptr, *d_r = nullptr, *d_p = nullptr, *d_t = nullptr;
+  double *d_ppt = nullptr, *d_prr = nullptr;
+  CgState *d_st = nullptr;
+  cudaError_t e = bf.up(&d_b, b, (size_t)n, st, A->device);
+  if (e == cudaSuccess) e = bf.up(&d_d, add_to_diag, (size_t)diag_len, st, A->device);
+  if (e == cudaSuccess) e = bf.alloc(&d_x, (size_t)n, A->device, st);
+  if (e == cudaSuccess) e = bf.alloc(&d_r, (size_t)n, A->device, st);
+  if (e == cudaSuccess) e = bf.alloc(&d_p, (size_t)n, A->device, st);
+  if (e == cudaSuccess) e = bf.alloc(&d_t, (size_t)n, A->device, st);
+  if (e == cudaSuccess) e = bf.alloc(&d_ppt, (size_t)nch, A->device, st);
+  if (e == cudaSuccess) e = bf.alloc(&d_prr, (size_t)nch, A->device, st);
+  if (e == cudaSuccess) e = bf.alloc(&d_st, 1, A->device, st);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    cudaStreamSynchronize(st);
+    return fail(e == cudaErrorMemoryAllocation ? BSG_ERR_ALLOC : BSG_ERR_CUDA, "solver state (%s)", cudaGetErrorString(e));
+  }
+  k_cg_init<<<nch, CG_DT, 0, st>>>(d_b, n, d_x, d_r, d_p, d_prr);
+  k_cg_init_fold<<<1, 32, 0, st>>>(d_prr, nch, d_st);
+  count_launch(2);
+  BSG_CUDA(cudaGetLastError());
+  CgState hs;
+  BSG_CUDA(cudaMemcpyAsync(&hs, d_st, sizeof hs, cudaMemcpyDeviceToHost, st));
+  BSG_CUDA(cudaStreamSynchronize(st));
+  const double rhs2 = hs.rhs2;
+  if (rhs2 == 0) {  // x = 0, no iteration, error 0
+    memset(x, 0, (size_t)n * sizeof(double));
+    *iters = 0, *error = 0;
+    return BSG_OK;
+  }
+  const double threshold = std::max(tol * tol * rhs2, DBL_MIN);
+  int it = 0;
+  if (hs.rn2 >= threshold) {
+    int nsm = 132;
+    cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, A->device);
+    const int mgrid = (int)std::min<long long>(((long long)n * 32 + CG_MT - 1) / CG_MT, (long long)nsm * (2048 / CG_MT));
+    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+    BSG_CUDA(cudaEventCreate(&ev0));
+    e = cudaEventCreate(&ev1);
+    if (e == cudaSuccess) e = cudaEventRecord(ev0, st);
+    while (e == cudaSuccess && it < maxiter && !hs.done) {
+      const int end = std::min(maxiter, it + CG_BLOCK);
+      count_launch(4 * (end - it));
+      for (; it < end; it++) {
+        k_cg_matvec<<<mgrid, CG_MT, 0, st>>>(A->p, A->rows, A->first_i, A->x, n, d_d, diag_len, d_p, d_t, d_st);
+        k_cg_pt<<<nch, CG_DT, 0, st>>>(d_p, d_t, n, d_ppt, d_st);
+        k_cg_update<<<nch, CG_DT, 0, st>>>(d_p, d_t, n, d_x, d_r, d_ppt, nch, d_prr, d_st, it);
+        k_cg_direction<<<nch, CG_DT, 0, st>>>(d_r, n, d_p, d_prr, nch, threshold, d_st, it);
+      }
+      e = cudaGetLastError();
+      if (e == cudaSuccess) e = cudaMemcpyAsync(&hs, d_st, sizeof hs, cudaMemcpyDeviceToHost, st);
+      if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    }
+    if (e == cudaSuccess) e = cudaEventRecord(ev1, st);
+    if (e == cudaSuccess) e = cudaEventSynchronize(ev1);
+    float ms = 0;
+    if (e == cudaSuccess) e = cudaEventElapsedTime(&ms, ev0, ev1);
+    A->last_solve_ms = ms;
+    cudaEventDestroy(ev0);
+    if (ev1) cudaEventDestroy(ev1);
+    if (e != cudaSuccess) return cuda_fail(e, "conjugate gradient");
+  }
+  BSG_CUDA(cudaMemcpyAsync(x, d_x, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, st));
+  BSG_CUDA(cudaStreamSynchronize(st));
+  *iters = hs.done ? hs.iters : it;  // maxiter when the threshold was never reached
+  *error = sqrt(hs.rn2 / rhs2);
+  return BSG_OK;
+}
+
+double bsg_sfbm_last_solve_ms(const bsg_sfbm *A) { return A ? A->last_solve_ms : -1.0; }
 
 }  // extern "C"

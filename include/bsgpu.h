@@ -256,6 +256,17 @@ int bsg_sfbm_ld_scores(bsg_sfbm *s, const int *ind_sub, int m, double *out);
 int bsg_lassosum2(bsg_sfbm *corr, const double *beta_hat, int m, const int *ind_sub, int ngrid, const double *lambda,
                   const double *delta_plus_one, double dfmax, int maxiter, double tol, double *beta_est, int *num_iter,
                   double *seconds);
+/* bigsparser::sp_solve_sym (called at R/LDpred2.R:38-39): x solving (A + diag(d)) x = b, A the n x n SFBM as stored, by
+ * Eigen's ConjugateGradient with the identity preconditioner from x = 0, every sum in one fixed order (DESIGN.md §4.13).
+ * d has length diag_len, 1 or n.  iters and error are Eigen's ConjugateGradient::iterations() / error(): the iteration
+ * that reached |r|^2 < max(tol^2 |b|^2, DBL_MIN) (not counted) or maxiter, and sqrt(|r|^2 / |b|^2); b = 0 gives x = 0,
+ * iters 0 and error 0.  A singular or indefinite system is not special-cased (error may be NaN).  A non-square handle or
+ * diag_len not in {1, n}: BSG_ERR_DIM; tol < 0, maxiter < 0 or a null pointer: BSG_ERR_ARG. */
+int bsg_sfbm_solve(bsg_sfbm *A, const double *b, const double *add_to_diag, int diag_len, double tol, int maxiter,
+                   double *x, int *iters, double *error);
+/* device time in ms (CUDA events) of the iterations of the last bsg_sfbm_solve on this handle, no-op launches after
+ * convergence included; 0 when it ran none */
+double bsg_sfbm_last_solve_ms(const bsg_sfbm *A);
 
 /* ---- near-independent LD blocks (snp_ldsplit, R/split-LD.R:99-138) -------------------------------------------------- */
 /* Matrix::tril(corr) staged to HBM once: m x m lower triangle in CSC, p[m + 1] (non-decreasing, p[0] = 0), rows i
