@@ -21,6 +21,7 @@ and error behaviour, so the parity tests read like the reference's testthat file
     snp_ldsplit / get_L / get_C   R/split-LD.R:3-40,99-138, src/split-LD.cpp:15-61,65-145,149-182
     sp_solve_sym / snp_ldpred2_inf   bigsparser's conjugate-gradient solve, R/LDpred2.R:27-42
     snp_ldsc / snp_ldsc2   R/ldsc.R:1-224 (host NumPy; the LD scores of snp_ldsc2 come from ld_scores_sfbm)
+    snp_PRS / snp_grid_PRS   R/PRS.R:36-76, R/SCT.R:201-246 (bsg_prs_grid: every keep set of a chromosome in one call)
 
 Everything computes on the GPU through libbsgpu; there is no CPU path here (LD score regression, a few
 weighted least-squares fits on per-variant vectors, runs on the host).
@@ -1703,3 +1704,121 @@ def get_C(L, min_size, max_size, max_K, max_cost, pos_scaled, device=0):
     check(lib().bsg_ldsplit_costs(m, lp.ctypes.data_as(_lib.c_i64_p), _pi(_i32(a.indices)), _pd(_f64(a.data)), int(min_size),
                                   int(max_size), K, float(max_cost), _pd(pos), int(device), _pd(Cm), _pi(best)))
     return {"C": Cm, "best_ind": best}
+
+
+# ---- C+T scores (snp_PRS, snp_grid_PRS) -----------------------------------------------------------------------------------
+
+class PRSScores(np.ndarray):
+    """snp_PRS's result: the nr x nthr score matrix, with the thresholds as `thr_list` (R's column names)."""
+
+    thr_list = None
+
+
+class GridPRS(np.ndarray):
+    """snp_grid_PRS's result: the nr x (keep sets x thresholds) score matrix (an np.memmap underneath when a backingfile
+    was given), with the attributes lpS, grid_lpS_thr, betas and all_keep of R/SCT.R:239-245."""
+
+    lpS = grid_lpS_thr = betas = all_keep = None
+
+
+def _prs_call(G, ind_row, sets, beta_cat, same_cat, lpS_cat, thr, out):
+    """One bsg_prs_grid call: keep sets `sets` (1-based column arrays) into the column-major block `out`."""
+    lens = _i32([len(s) for s in sets])
+    cols = _i32(np.concatenate([np.asarray(s).reshape(-1) for s in sets])) if sets else np.zeros(0, dtype=np.int32)
+    same = None if same_cat is None else _i32(same_cat)
+    lp = None if lpS_cat is None else _f64(lpS_cat)
+    th = None if thr is None else _f64(thr)
+    nthr = 1 if thr is None else th.size
+    check(lib().bsg_prs_grid(G._h, _pi(ind_row), ind_row.size, len(sets), _pi(lens), _pi(cols), _pd(_f64(beta_cat)),
+                             _pi(same), _pd(lp), nthr, _pd(th), int(out.dtype == np.float64),
+                             C.c_void_p(out.ctypes.data) if out.size else None))
+
+
+def _check_lpS(lpS, name):
+    if np.any(np.isnan(lpS)):
+        raise ValueError("%s must not have missing values." % name)
+    if np.any(lpS < 0):
+        raise ValueError("%s should have only non-negative values." % name)
+
+
+def snp_PRS(G, betas_keep, ind_test=..., ind_keep=..., same_keep=None, lpS_keep=None, thr_list=0):
+    """R/PRS.R:36-76 on a hard-call handle: the scores of ind_test for every threshold of thr_list (columns in the
+    caller's order), one bsg_prs_grid call.  lpS_keep None or thr_list identical to 0: one column over every kept SNP."""
+    import sys
+
+    _assert_bed(G)
+    ind_test = G.rows_along() if ind_test is ... else _i32(ind_test)
+    ind_keep = G.cols_along() if ind_keep is ... else _i32(ind_keep)
+    betas_keep = _f64(betas_keep)
+    if same_keep is None:
+        same_keep = np.ones(ind_keep.size, dtype=bool)
+    else:
+        same_keep = np.asarray(same_keep)
+        if same_keep.dtype == object and any(s is None for s in same_keep.ravel()):
+            raise ValueError("'same.keep' should have no missing value.")
+        if same_keep.dtype != np.bool_:
+            raise TypeError("'same.keep' should be of type 'logical'.")
+    _assert_lengths(same_keep, ind_keep)
+    _assert_lengths(betas_keep, ind_keep)
+    thr = np.asarray(thr_list)
+    disabled = lpS_keep is None or (thr.size == 1 and thr.dtype.kind in "if" and thr.item() == 0)
+    if disabled:
+        print("'lpS.keep' or 'thr.list' was not specified. Thresholding disabled.", file=sys.stderr)
+        lp, th = None, None
+    else:
+        lp = _f64(lpS_keep)
+        _assert_lengths(lp, ind_keep)
+        _check_lpS(lp, "'lpS.keep'")
+        th = _f64(thr.reshape(-1))
+    out = np.empty((ind_test.size, 1 if th is None else th.size), order="F")
+    _prs_call(G, ind_test, [ind_keep], betas_keep, same_keep.astype(np.int32), lp, th, out)
+    out = out.view(PRSScores)
+    out.thr_list = None if th is None else th
+    return out
+
+
+def snp_grid_PRS(G, all_keep, betas, lpS, n_thr_lpS=50, grid_lpS_thr=None, ind_row=..., backingfile=None, type="float",
+                 ncores=1):
+    """R/SCT.R:201-246: C+T scores of every keep set of snp_grid_clumping (a GridClumping, or a list per chromosome of
+    1-based index arrays) at every threshold; column (ic - 1) n_thr + t is keep set ic (chromosome-major) at threshold t.
+    One bsg_prs_grid call per chromosome.  backingfile: the matrix is an np.memmap of backingfile + '.bk' (R's FBM file)."""
+    _assert_bed(G)
+    betas, lpS = _f64(betas), _f64(lpS)
+    _assert_lengths(G.cols_along(), betas)
+    _assert_lengths(G.cols_along(), lpS)
+    if type not in ("float", "double"):
+        raise ValueError("'type' should be one of \"float\", \"double\".")
+    if grid_lpS_thr is None:
+        grid_lpS_thr = 0.9999 * seq_log(max(0.1, float(np.nanmin(lpS))), float(np.nanmax(lpS)), n_thr_lpS)
+    thr = _f64(np.asarray(grid_lpS_thr, dtype=np.float64).reshape(-1))
+    disabled = thr.size == 1 and thr[0] == 0  # snp_PRS's identical(thr.list, 0): one column over every kept SNP
+    ind_row = G.rows_along() if ind_row is ... else _i32(ind_row)
+    chroms = [[np.asarray(s, dtype=np.int64).reshape(-1) for s in chrom] for chrom in all_keep]
+    cats = []
+    for chrom in chroms:  # every chromosome is checked before the result file is created
+        cat = np.concatenate(chrom) if chrom else np.zeros(0, dtype=np.int64)
+        if np.any((cat < 1) | (cat > G.ncol)):
+            raise IndexError("subscript out of bounds")
+        if not disabled:
+            _check_lpS(lpS[cat - 1], "'lpS.keep'")
+        cats.append(cat)
+    nsets = sum(len(c) for c in chroms)
+    shape = (ind_row.size, nsets * thr.size)
+    dtype = np.float32 if type == "float" else np.float64
+    if backingfile is None:
+        out = np.empty(shape, dtype=dtype, order="F")
+    else:
+        out = np.memmap(backingfile + ".bk", dtype=dtype, mode="w+", shape=shape, order="F")
+    col = 0
+    for chrom, cat in zip(chroms, cats):
+        if not chrom:
+            continue
+        ncol = len(chrom) * thr.size
+        _prs_call(G, ind_row, chrom, betas[cat - 1], None, None if disabled else lpS[cat - 1], None if disabled else thr,
+                  out[:, col:col + ncol])
+        col += ncol
+    if backingfile is not None:
+        out.flush()
+    res = out.view(GridPRS)
+    res.lpS, res.grid_lpS_thr, res.betas, res.all_keep = lpS, thr, betas, all_keep
+    return res

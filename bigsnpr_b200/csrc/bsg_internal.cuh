@@ -291,6 +291,8 @@ int fbm_nan_rows(const uint8_t *d_na, int nr, int K, double *d_XV, cudaStream_t 
 // bsg_pmv.cu: the vector preparation these kernels share with the 2-bit ones
 int dosage_prep_cols(bsg_view *v, const double *x_dev, cudaStream_t s);
 int dosage_prep_rows(bsg_view *v, const double *x_dev, long long *Q, cudaStream_t s);
+// bsg_prs.cu: digits of one keep set's weights x[len] (len a multiple of 32) in k_pmvT's step order, exponent into *sc
+int prs_prep(const double *x_dev, int len, pmv::Scal *sc, uint8_t *dig, cudaStream_t s);
 
 // ---- bsg_la.cu: the Lanczos driver over one or several column shards (one replica of the recurrence per shard) ----
 struct SvdShard {

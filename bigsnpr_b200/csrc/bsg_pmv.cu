@@ -1673,6 +1673,18 @@ int bsg::dosage_prep_rows(bsg_view *v, const double *x_dev, long long *Q, cudaSt
   return BSG_OK;
 }
 
+// C+T scores (bsg_prs.cu): every entry of a keep set is its own line, so one quantised value per digit block (hb = 0)
+int bsg::prs_prep(const double *x_dev, int len, pmv::Scal *sc, uint8_t *dig, cudaStream_t s) {
+  using namespace pmv;
+  BSG_CUDA(cudaMemsetAsync(sc, 0, sizeof(Scal), s));
+  k_prep1<<<SUMCZ_BLOCKS, 256, 0, s>>>(0, x_dev, nullptr, nullptr, len, 0, sc);
+  pmvt::k_quantT<1><<<launch_cap(len, 256, 1184), 256, 0, s>>>(0, x_dev, nullptr, nullptr, nullptr, len, len, sc, dig, nullptr,
+                                                         nullptr, nullptr, 0);
+  count_launch(2);
+  BSG_CUDA(cudaGetLastError());
+  return BSG_OK;
+}
+
 // X~ x : lines = samples of copy B, contraction over SNP columns.  comm != null: the result is summed over the column
 // shards of the communicator (every rank receives the full n-vector).
 int bsg::view_prodvec_comm(bsg_view *v, const double *x_dev, double *out_dev, cudaStream_t s, bsg_comm *comm) {

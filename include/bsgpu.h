@@ -230,6 +230,27 @@ int bsg_grid_clumping_chr(bsg_bed *h, const int *ind_row, int nr, const int *ind
                           const double *sumX, const double *denoX, int nsub, const int *sub_len, const int *sub_col,
                           const int *sub_ord, int npt, const double *thr_r2, const double *size_bp, int *keep);
 
+/* snp_PRS with thresholding (R/PRS.R:36-76) for nsets keep sets at once: what snp_grid_PRS (R/SCT.R:201-246) computes
+ * for one chromosome.  Set c has set_len[c] entries, concatenated over the sets in cols (1-based columns, repeats
+ * allowed), beta, same (NULL = all TRUE; 0 / 1) and lpS.  Thresholds are visited in stable decreasing order; an entry
+ * joins at the first one its lpS exceeds (strict >), and column c * nthr + t of out (nr x nsets * nthr, column-major,
+ * float rounded to nearest when out_double = 0, else double) is set c at thr[t]: prodVecRev summed over every entry
+ * joined so far.  thr = NULL with nthr = 1 disables thresholding (one column over all entries, lpS unused).
+ * The scores are exact integer sums of the codes times the 61-bit fixed-point weights (one quantisation per set,
+ * reversed alleles as (g - 2) Q), with one fp64 sum of 8 digit slices per output.  A row holding an NA code in a
+ * column joined so far is NaN (R: last + NA stays NA).  A set holding a non-finite beta is computed by R's loop in
+ * fp64 instead (sum(betas[!same]) in double, R sums in long double).  ind_row: 1-based, repeats allowed, NULL = all.
+ * A NaN or negative lpS of an entry, a NaN threshold, same not in {0, 1} or bad lengths: BSG_ERR_ARG (R's result for a
+ * NaN lpS is an NA index, deliberately refused here); columns or rows out of range: BSG_ERR_BOUNDS.  Dosage tables
+ * (bsg_dosage_scale D > 0) use the value bytes D x code and divide the slice sum by D once; other FBM.code256 tables:
+ * BSG_ERR_TYPE; scratch and output larger than the free device memory:
+ * BSG_ERR_ALLOC with the bytes needed, before any allocation. */
+int bsg_prs_grid(bsg_bed *h, const int *ind_row, int nr, int nsets, const int *set_len, const int *cols,
+                 const double *beta, const int *same, const double *lpS, int nthr, const double *thr, int out_double,
+                 void *out);
+/* device time in ms (CUDA events) of the last bsg_prs_grid, quantisation to the gathered output, copies excluded */
+double bsg_prs_last_ms(void);
+
 /* ---- sparse LD matrix (bigsparser's SFBM) and summary-statistics PRS -------------------------------------- */
 /* as_SFBM(corr[, compact]) staged to HBM once, in bigsparser's storage as bigsnpr reads it (src/ld-scores-sfbm.cpp:14-66):
  *   - p: ncol + 1 doubles, non-decreasing integers starting at 0 (X$p);
