@@ -285,12 +285,12 @@ __global__ void k_expand_weighted(const uint8_t *__restrict__ P, int64_t stride,
   }
 }
 
-// digits in plain order: dig[s * dig_stride + k] = digit s (dbits wide) of rint(W[k] * 2^e); zero for k >= len
-__global__ void k_weight_digits_plain(const double *__restrict__ W, int64_t len, int64_t dig_stride, int nslices, int e, int dbits,
-                                      uint8_t *__restrict__ dig) {
+// digits in plain order: dig[s * dig_stride + k] = digit s (dbits wide) of rint(W[k] * 2^e); zero outside [lo, hi)
+__global__ void k_weight_digits_plain(const double *__restrict__ W, int64_t lo, int64_t hi, int64_t dig_stride, int nslices, int e,
+                                      int dbits, uint8_t *__restrict__ dig) {
   for (int64_t k = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; k < dig_stride; k += (int64_t)gridDim.x * blockDim.x) {
     unsigned long long v = 0;
-    if (k < len) v = (unsigned long long)__double2ll_rn(scalbn(W[k], e));
+    if (k >= lo && k < hi) v = (unsigned long long)__double2ll_rn(scalbn(W[k], e));
     for (int s = 0; s < nslices; s++) {
       dig[(int64_t)s * dig_stride + k] = (uint8_t)(v & ((1ull << dbits) - 1ull));
       v >>= dbits;
@@ -350,16 +350,19 @@ bool gramt_enabled() {
 
 // ---------------------------------------------------------------------------------------------------------------------------
 // GRM: K (pre-zeroed, nr x nr column-major, filled for i >= j) += sum_k w-weighted integer Grams of the packed sample-major
-// lines P.  Ws = {W1, W2', W3} (device, length nc), wmax their maxima, na[i] = 1 if line i holds a missing value.
+// lines P.  Ws = {W1, W2', W3} (device, length nc), wmax their maxima over [klo, khi), na[i] = 1 if line i holds a missing
+// value.  Only the weights of the columns [klo, khi) (one weight class, tcrossprod_impl) are quantised; the contraction runs
+// over that range rounded out to whole 128-code k-blocks, where the digits of the neighbouring columns are zero.
 // Columns are processed in blocks of at most KBLK codes: expand -> one launch per plane product -> K accumulates in fp64.
 // ---------------------------------------------------------------------------------------------------------------------------
 int gramt_grm(const uint8_t *P, int64_t stride, int nr, int nc, const double *const Ws[3], const double wmax[3],
-              const uint8_t *na, int nslices, double *K, int64_t ldk, int device, cudaStream_t s) {
+              const uint8_t *na, int nslices, double *K, int64_t ldk, int device, cudaStream_t s, int64_t klo, int64_t khi) {
   using namespace gt;
   if (nslices > NBMAX) nslices = NBMAX;
   const int dbits = 7;
   const int64_t KBLK = 262144;  // 2 * 254 * 262144 < 2^31: int32 accumulators cannot overflow within a block
-  const int64_t kblk = std::min<int64_t>(KBLK, round_up(nc, BK));
+  const int64_t kb0 = klo / BK * BK, kb1 = std::min<int64_t>(nc, round_up(khi, BK));
+  const int64_t kblk = std::min<int64_t>(KBLK, round_up(kb1 - kb0, BK));
   const int64_t lines_pad = round_up(nr, 256);
   bool any_na = false;
   for (int i = 0; i < nr; i++) any_na |= na[i] != 0;
@@ -389,7 +392,7 @@ int gramt_grm(const uint8_t *P, int64_t stride, int nr, int nc, const double *co
     int ex = 0;
     if (wmax[wv] > 0) frexp(wmax[wv], &ex);
     const int e = dbits * nslices - 1 - ex;
-    k_weight_digits_plain<<<grid_cap(dig_stride), 256, 0, s>>>(Ws[wv], nc, dig_stride, nslices, e, dbits, dig[wv]);
+    k_weight_digits_plain<<<grid_cap(dig_stride), 256, 0, s>>>(Ws[wv], klo, khi, dig_stride, nslices, e, dbits, dig[wv]);
     count_launch();
     for (int sl = 0; sl < NBMAX; sl++) scale[wv][sl] = sl < nslices ? ldexp(1.0, dbits * sl - e) : 0.0;
   }
@@ -420,8 +423,8 @@ int gramt_grm(const uint8_t *P, int64_t stride, int nr, int nc, const double *co
   if (nt_na) BSG_CUDA(cudaMemcpyAsync(d_tiles + nt_all, tiles_na.data(), nt_na * sizeof(GtTile), cudaMemcpyHostToDevice, s));
   BSG_CUDA(cudaStreamSynchronize(s));  // host vectors go out of scope at return; also orders the tile upload
 
-  for (int64_t k0 = 0; k0 < nc; k0 += kblk) {
-    const int64_t klen = std::min<int64_t>(kblk, nc - k0);
+  for (int64_t k0 = kb0; k0 < kb1; k0 += kblk) {
+    const int64_t klen = std::min<int64_t>(kblk, kb1 - k0);
     const int64_t pitch = round_up(klen, BK);
     CUtensorMap mAa, mAn, mB;
     BSG_TRY(make_map(&mAa, Aa, lines_pad, pitch, BM));

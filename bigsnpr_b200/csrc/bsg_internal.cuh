@@ -266,7 +266,7 @@ int dosage_pair_levels(bsg_bed *h, const int *d_row, int nr, const int *d_col, i
 namespace gram { struct Tile; }
 bool gramt_enabled();  // BSG_GRAM_TMA=0 selects the round-1 kernels (in-kernel expansion) for cross-checks
 int gramt_grm(const uint8_t *P, int64_t stride, int nr, int nc, const double *const Ws[3], const double wmax[3],
-              const uint8_t *na, int nslices, double *K, int64_t ldk, int device, cudaStream_t s);
+              const uint8_t *na, int nslices, double *K, int64_t ldk, int device, cudaStream_t s, int64_t klo, int64_t khi);
 int gramt_cor(const uint8_t *M, int64_t stride, int nlines, const gram::Tile *tiles, int ntiles, int *d_sums, int device,
               cudaStream_t s, bool *done);
 // TMA map over rows x pitch bytes: 128 B x box_rows boxes, 128-byte swizzle, zero fill out of bounds

@@ -312,8 +312,9 @@ __global__ void __launch_bounds__(THREADS, 1) k_wgram(const WArgs a) {
   }
 }
 
-// weight digits in fragment order: byte ((chunk*4 + q)*4 + w)*16 + c*4 + r  <->  k = chunk*256 + (4q+w)*16 + 4r + c
-__global__ void k_weight_digits(const double *__restrict__ W, int len, int nchunks, int nslices, int e, int dbits,
+// weight digits in fragment order: byte ((chunk*4 + q)*4 + w)*16 + c*4 + r  <->  k = chunk*256 + (4q+w)*16 + 4r + c;
+// zero outside the columns [lo, hi) of one weight class
+__global__ void k_weight_digits(const double *__restrict__ W, int lo, int hi, int nchunks, int nslices, int e, int dbits,
                                 uint8_t *__restrict__ dig) {
   int64_t total = (int64_t)nchunks * 256;
   for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
@@ -321,7 +322,7 @@ __global__ void k_weight_digits(const double *__restrict__ W, int len, int nchun
     const int c = byte >> 2, r = byte & 3, w = unit & 3, q = unit >> 2;
     const int64_t k = (int64_t)chunk * 256 + (4 * q + w) * 16 + 4 * r + c;
     unsigned long long v = 0;
-    if (k < len) v = (unsigned long long)__double2ll_rn(scalbn(W[k], e));
+    if (k >= lo && k < hi) v = (unsigned long long)__double2ll_rn(scalbn(W[k], e));
     for (int sl = 0; sl < nslices; sl++) {
       dig[(int64_t)sl * total + t] = (uint8_t)(v & ((1ull << dbits) - 1ull));
       v >>= dbits;
@@ -876,16 +877,79 @@ static int tcrossprod_impl(bsg_bed *h, const int *ind_row, int nr, const int *in
   k_grm_weights<<<(nc + 255) / 256, 256, 0, s>>>(d_c, d_s, nc, W1, W2p, W3, w2, d_stats);
   count_launch();
   double stats[8];
-  std::vector<double> hW3(nc);
+  std::vector<double> hW1(nc), hW3(nc);
   BSG_CUDA(cudaMemcpyAsync(stats, d_stats, sizeof stats, cudaMemcpyDeviceToHost, s));
+  BSG_CUDA(cudaMemcpyAsync(hW1.data(), W1, (size_t)nc * sizeof(double), cudaMemcpyDeviceToHost, s));
   BSG_CUDA(cudaMemcpyAsync(hW3.data(), W3, (size_t)nc * sizeof(double), cudaMemcpyDeviceToHost, s));
   BSG_CUDA(cudaStreamSynchronize(s));
   if (stats[4] != 0.0) return tcrossprod_dsyrk(h, ind_row, nr, ind_col, nc, center, scale, K, K_dev);
   double sumW3 = 0;
   for (int j = 0; j < nc; j++) sumW3 += hW3[j];
 
-  // ---- the sub-matrix X[ind_row, ind_col] as dense sample-major lines
-  const bool ident = (!ind_row || [&] { if (nr != h->n) return false; for (int i = 0; i < nr; i++) if (ind_row[i] != i + 1) return false; return true; }()) &&
+  // ---- weight classes.  One exponent per weight vector leaves a column whose W1 lies 2^b below the maximum only
+  // 28 - b of the 28 bits (a singleton's W1 = 1 / (2 p (1 - p)) is ~n times a common variant's).  The columns are
+  // binned by W1: class c holds max W1 / 16^(c+1) < W1 <= max W1 / 16^c (W1 = 0: class 0), so every W1 of a class is
+  // within a factor 16 of the class maximum and keeps at least 24 bits; W2' = c W1 and W3 = c^2 W1 follow for centers
+  // in [0, 2].  Each class is quantised with its own exponents and folded into K in turn, over the columns of the
+  // compacted copy stably sorted by class.  One class is the unsplit computation, byte for byte.
+  struct WClass {
+    int lo, hi;  // columns [lo, hi) of the (sorted) copy
+    double wmax[3];
+  };
+  std::vector<WClass> classes;
+  std::vector<int> pcol;  // 1-based columns sorted by class (several classes only)
+  const double *Wg[3] = {W1, W2p, W3};
+  {
+    const double w1max = stats[0];
+    bool one = true;
+    for (int j = 0; j < nc && one; j++) one = !(hW1[j] > 0 && hW1[j] * 16.0 <= w1max);  // exact: a power of two
+    if (one) {
+      classes.push_back(WClass{0, nc, {stats[0], stats[1], stats[2]}});
+    } else {
+      int exmax = 0;
+      frexp(w1max, &exmax);
+      std::vector<int> cls(nc), perm(nc);
+      for (int j = 0; j < nc; j++) {
+        int c = 0;
+        if (hW1[j] > 0) {  // floor(log2(max / W1) / 4), from the exponents and corrected by one exact comparison each way
+          int ex = 0;
+          frexp(hW1[j], &ex);
+          c = (exmax - ex) / 4;
+          if (ldexp(hW1[j], 4 * (c + 1)) <= w1max) c++;
+          else if (c > 0 && ldexp(hW1[j], 4 * c) > w1max) c--;
+        }
+        cls[j] = c;
+        perm[j] = j;
+      }
+      std::stable_sort(perm.begin(), perm.end(), [&](int x, int y) { return cls[x] < cls[y]; });
+      std::vector<double> hW2p(nc), hw[3];
+      BSG_CUDA(cudaMemcpyAsync(hW2p.data(), W2p, (size_t)nc * sizeof(double), cudaMemcpyDeviceToHost, s));
+      BSG_CUDA(cudaStreamSynchronize(s));
+      const std::vector<double> *src[3] = {&hW1, &hW2p, &hW3};
+      pcol.resize(nc);
+      for (int wv = 0; wv < 3; wv++) hw[wv].resize(nc);
+      for (int k = 0; k < nc; k++) {
+        const int j = perm[k];
+        pcol[k] = ind_col ? ind_col[j] : j + 1;
+        for (int wv = 0; wv < 3; wv++) hw[wv][k] = (*src[wv])[j];
+        if (k == 0 || cls[j] != cls[perm[k - 1]]) classes.push_back(WClass{k, k, {0.0, 0.0, 0.0}});
+        WClass &c = classes.back();
+        c.hi = k + 1;
+        for (int wv = 0; wv < 3; wv++) c.wmax[wv] = std::max(c.wmax[wv], hw[wv][k]);
+      }
+      for (int wv = 0; wv < 3; wv++) {
+        double *d = nullptr;
+        BSG_TRY(mem.alloc(&d, nc));
+        BSG_CUDA(cudaMemcpyAsync(d, hw[wv].data(), (size_t)nc * sizeof(double), cudaMemcpyHostToDevice, s));
+        Wg[wv] = d;
+      }
+      BSG_CUDA(cudaStreamSynchronize(s));  // the host copies go out of scope
+    }
+  }
+
+  // ---- the sub-matrix X[ind_row, ind_col] as dense sample-major lines (columns sorted by class)
+  const bool ident = pcol.empty() &&
+                     (!ind_row || [&] { if (nr != h->n) return false; for (int i = 0; i < nr; i++) if (ind_row[i] != i + 1) return false; return true; }()) &&
                      (!ind_col || [&] { if (nc != h->m) return false; for (int j = 0; j < nc; j++) if (ind_col[j] != j + 1) return false; return true; }());
   const uint8_t *P = h->B;
   int64_t stride = h->strideB;
@@ -894,7 +958,7 @@ static int tcrossprod_impl(bsg_bed *h, const int *ind_row, int nr, const int *in
   if (!ident) {
     const int *d_row = nullptr, *d_col = nullptr;
     BSG_TRY(upload_index(h, ind_row, nr, h->n, h->w_idx_row, &d_row));
-    BSG_TRY(upload_index(h, ind_col, nc, h->m, h->w_idx_col, &d_col));
+    BSG_TRY(upload_index(h, pcol.empty() ? ind_col : pcol.data(), nc, h->m, h->w_idx_col, &d_col));
     stride = round_up(((int64_t)nc + 3) / 4, CHUNK);
     uint8_t *Pc = nullptr;
     BSG_TRY(mem.alloc(&Pc, (size_t)stride * nr));
@@ -916,32 +980,35 @@ static int tcrossprod_impl(bsg_bed *h, const int *ind_row, int nr, const int *in
   if (!K_dev) BSG_TRY(mem.alloc(&dK, (size_t)nr * nr));
   BSG_CUDA(cudaMemsetAsync(dK, 0, (size_t)nr * nr * sizeof(double), s));
   if (gramt_enabled() && nslices <= 4) {
-    // TMA-fed wgmma tiles over operands expanded once to uint8 (bsg_gramt.cu): all digit slices in one launch
-    const double *Ws3[3] = {W1, W2p, W3};
-    const double wmax[3] = {stats[0], stats[1], stats[2]};
-    BSG_TRY(gramt_grm(P, stride, nr, nc, Ws3, wmax, na.data(), nslices, dK, nr, h->device, s));
+    // TMA-fed wgmma tiles over operands expanded once to uint8 (bsg_gramt.cu): all digit slices in one launch per
+    // k-block and product, over the k-range of each weight class in turn
+    for (const WClass &c : classes)
+      BSG_TRY(gramt_grm(P, stride, nr, nc, Wg, c.wmax, na.data(), nslices, dK, nr, h->device, s, c.lo, c.hi));
   } else {
-  // ---- weight digits (base 64, nslices digits) in fragment order
+  // ---- weight digits (base 2^dbits, nslices digits) in fragment order, recomputed per class
   WArgs a;
   a.P = P;
   a.stride = stride;
   a.nlines = nr;
   a.nchunks = nchunks;
   a.nslices = nslices;
-  const double *Ws[3] = {W1, W2p, W3};
   const int dbits = nc <= 4000000 ? 7 : 6;  // longer sweeps keep the int32 head-room with 6-bit digits (2 * 126 * m < 2^31 up to 8.5 M)
+  uint8_t *dg[3] = {nullptr, nullptr, nullptr};
   for (int wv = 0; wv < 3; wv++) {
-    uint8_t *dg = nullptr;
-    BSG_TRY(mem.alloc(&dg, (size_t)nslices * nchunks * 256));
-    int ex = 0;
-    if (stats[wv] > 0) frexp(stats[wv], &ex);
-    const int e = dbits * nslices - 1 - ex;
-    k_weight_digits<<<(int)std::min<int64_t>(((int64_t)nchunks * 256 + 255) / 256, 132 * 16), 256, 0, s>>>(Ws[wv], nc, nchunks,
-                                                                                                        nslices, e, dbits, dg);
-    count_launch();
-    a.dig[wv] = dg;
-    for (int sl = 0; sl < nslices; sl++) a.scale[wv][sl] = ldexp(1.0, dbits * sl - e);
+    BSG_TRY(mem.alloc(&dg[wv], (size_t)nslices * nchunks * 256));
+    a.dig[wv] = dg[wv];
   }
+  auto class_digits = [&](const WClass &c) {
+    for (int wv = 0; wv < 3; wv++) {
+      int ex = 0;
+      if (c.wmax[wv] > 0) frexp(c.wmax[wv], &ex);
+      const int e = dbits * nslices - 1 - ex;
+      k_weight_digits<<<(int)std::min<int64_t>(((int64_t)nchunks * 256 + 255) / 256, 132 * 16), 256, 0, s>>>(
+          Wg[wv], c.lo, c.hi, nchunks, nslices, e, dbits, dg[wv]);
+      count_launch();
+      for (int sl = 0; sl < nslices; sl++) a.scale[wv][sl] = ldexp(1.0, dbits * sl - e);
+    }
+  };
 
   // ---- tiles of the lower triangle
   static int use_t5 = -1;
@@ -965,8 +1032,11 @@ static int tcrossprod_impl(bsg_bed *h, const int *ind_row, int nr, const int *in
       }
     }
     const uint8_t *digs[3] = {a.dig[0], a.dig[1], a.dig[2]};
-    BSG_TRY(wgram5_launch(P, stride, nr, nslices, digs, (int64_t)nchunks * 256, a.scale, trip.data(), (int)(trip.size() / 3),
-                          dK, nr, s));
+    for (const WClass &c : classes) {
+      class_digits(c);
+      BSG_TRY(wgram5_launch(P, stride, nr, nslices, digs, (int64_t)nchunks * 256, a.scale, trip.data(), (int)(trip.size() / 3),
+                            dK, nr, s));
+    }
   } else {
     std::vector<WTile> tiles;
     for (int i0 = 0; i0 < nr; i0 += TM) {
@@ -981,9 +1051,12 @@ static int tcrossprod_impl(bsg_bed *h, const int *ind_row, int nr, const int *in
     a.tiles = d_tiles;
     a.K = dK;
     a.ldk = nr;
-    k_wgram<<<(unsigned)tiles.size(), THREADS, 0, s>>>(a);
-    count_launch();
-    BSG_CUDA(cudaGetLastError());
+    for (const WClass &c : classes) {
+      class_digits(c);
+      k_wgram<<<(unsigned)tiles.size(), THREADS, 0, s>>>(a);
+      count_launch();
+      BSG_CUDA(cudaGetLastError());
+    }
     BSG_CUDA(cudaStreamSynchronize(s));
   }
 

@@ -84,6 +84,39 @@ def main():
                           "cfg4_extrapolated_s": t * 1_000_000 / a.grm_m, "path": os.environ.get("BSG_GRM_DSYRK", "0"),
                           "slices": os.environ.get("BSG_GRM_SLICES", "8")}), flush=True)
         g.close()
+    # the same matrix with a caller's scaling that puts 1 % of the columns in rare-variant weight classes (cohort
+    # allele frequencies of 1e-3 and 1e-5): the columns are sorted by class and each class is folded in turn
+    g = B.Bed.synthetic(a.grm_n, a.grm_m, seed=20250928)
+    sc = B.bed_scaleBinom(g)
+    c, s = np.array(sc["center"]), np.array(sc["scale"])
+    rare = np.random.default_rng(1).choice(a.grm_m, a.grm_m // 100, replace=False)
+    pc = np.where(np.arange(rare.size) % 2 == 0, 1e-3, 1e-5)
+    c[rare], s[rare] = 2 * pc, np.sqrt(2 * pc * (1 - pc))
+    W1 = 1.0 / (s * s)
+    ncls = np.unique(np.floor(np.log2(W1.max() / W1) / 4)).size  # the class rule of bsg_la.cu tcrossprod_impl
+    t, _ = timeit(lambda: B.bed_tcrossprodSelf(g, fun_scaling=lambda *aa, **kw: {"center": c, "scale": s}))
+    print(json.dumps({"op": "bed_tcrossprodSelf", "n": a.grm_n, "m": a.grm_m, "na_rate": 0.0, "seconds": t,
+                      "rare_columns": int(rare.size), "weight_classes": int(ncls), "gpu": _gpu_name(),
+                      "power_limit_w": _power_limit()}), flush=True)
+    g.close()
+
+
+def _gpu_name():
+    import torch
+
+    return torch.cuda.get_device_name(0)
+
+
+def _power_limit():
+    """The enforced power limit of GPU 0 in W, read (not set) through nvidia-smi; None where it cannot be read."""
+    import subprocess
+
+    try:
+        r = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
+                           capture_output=True, text=True, timeout=30)
+        return float(r.stdout.strip().splitlines()[0])
+    except Exception:  # pragma: no cover
+        return None
 
 
 if __name__ == "__main__":
