@@ -383,12 +383,75 @@ __global__ void k_tcol(const double *__restrict__ hcoef, int cnt, double *__rest
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < cnt) tcol[i] = add ? tcol[i] + hcoef[i] : hcoef[i];
 }
-// scal[0] = |w| (the next off-diagonal entry, kept as beta of the last step), scal[1] = 1 / |w| (0 if w == 0)
-__global__ void k_norm_step(const double *__restrict__ h0, double *__restrict__ T, int ncv, int j, double *__restrict__ scal) {
-  const double nrm = sqrt(h0[0]);
+// Krylov breakdown: w kept less than this fraction of A v_j after the two Gram-Schmidt passes.  What is left is rounding
+// noise, and when that noise lies mostly in span(V) (exact per-line products of duplicated rows or columns keep it
+// there) the second pass removes it too and w / |w| is far from orthogonal to V.  Above the threshold two passes leave
+// w orthogonal to V to a few ulps.
+#define BSG_LANCZOS_BREAKDOWN 1e-13
+
+// scal[0] = |w| (beta of the step; that of the last step enters the residual estimates), scal[1] = 1 / |w| (0 if
+// w == 0), scal[2] = 1 on a breakdown of step j: beta = 0 and k_refill replaces w.  |A v_j|^2 = |w|^2 + |column j of T|^2.
+// The off-diagonal entry T[j, j+1] is not written here: column j + 1 of T is computed as Gram-Schmidt coefficients.
+__global__ void k_norm_step(const double *__restrict__ h0, const double *__restrict__ T, int ncv, int j, double *__restrict__ scal) {
+  double nrm = sqrt(h0[0]);
+  bool brk = false;
+  if (j >= 0) {
+    double hh = nrm * nrm;
+    for (int i = 0; i <= j; i++) hh += T[(size_t)j * ncv + i] * T[(size_t)j * ncv + i];
+    brk = nrm <= BSG_LANCZOS_BREAKDOWN * sqrt(hh);  // false for NaN: the host still sees a non-finite matrix
+  }
+  if (brk) nrm = 0;
   scal[0] = nrm;
   scal[1] = nrm > 0 ? 1.0 / nrm : 0.0;
-  if (j >= 0 && j + 1 < ncv) T[(size_t)(j + 1) * ncv + j] = nrm;
+  scal[2] = brk ? 1.0 : 0.0;
+}
+
+// deterministic block sum of a[i] * b[i] (one block, fixed thread -> element map); every thread gets the result
+__device__ double block_dot(const double *__restrict__ a, const double *__restrict__ b, int N, double *red) {
+  double acc = 0;
+  for (int i = threadIdx.x; i < N; i += blockDim.x) acc += a[i] * b[i];
+#pragma unroll
+  for (int o = 16; o; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = acc;
+  __syncthreads();
+  double t = 0;
+  for (int k = 0; k < (int)(blockDim.x >> 5); k++) t += red[k];
+  return t;
+}
+
+// after a breakdown (scal[2] set by k_norm_step): w = a fresh start vector (seeded), orthogonalised twice against
+// V[:, 0..cnt) and normalised through scal[1], like ARPACK's dgetv0.  One block; returns at once otherwise, so the
+// recurrence needs no host decision.  hbuf: cnt doubles of scratch.
+__global__ void __launch_bounds__(1024) k_refill(const double *__restrict__ V, int64_t ld, int cnt, int N, uint64_t seed,
+                                                 double *__restrict__ w, double *__restrict__ hbuf, double *__restrict__ scal) {
+  __shared__ double red[32];
+  if (scal[2] == 0.0) return;
+  for (int i = threadIdx.x; i < N; i += blockDim.x) {
+    uint64_t x = seed + 0x9E3779B97F4A7C15ull * (uint64_t)(i + 1);
+    x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
+    x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
+    x ^= x >> 31;
+    w[i] = ((double)(x >> 11) * (1.0 / 9007199254740992.0)) - 0.5;
+  }
+  __syncthreads();
+  const double n0 = sqrt(block_dot(w, w, N, red));
+  for (int pass = 0; pass < 2; pass++) {
+    for (int c = 0; c < cnt; c++) {
+      const double h = block_dot(V + (int64_t)c * ld, w, N, red);
+      if (threadIdx.x == 0) hbuf[c] = h;
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < N; i += blockDim.x) {
+      double acc = 0;
+      for (int c = 0; c < cnt; c++) acc += V[(int64_t)c * ld + i] * hbuf[c];
+      w[i] -= acc;
+    }
+    __syncthreads();
+  }
+  const double nrm = sqrt(block_dot(w, w, N, red));
+  // V spans the whole space (the last step of ncv == N): nothing is left, the vector stays zero
+  if (threadIdx.x == 0) scal[1] = nrm > 1e-8 * n0 ? 1.0 / nrm : 0.0;
 }
 __global__ void k_scale_copy_p(const double *__restrict__ src, const double *__restrict__ alpha, int N, double *__restrict__ dst) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -552,6 +615,10 @@ int lanczos_svd(std::vector<SvdShard> &sh, const int *ind_row, int nr, int ncol_
       dots(g, rep[g].wv, 1, rep[g].wv);
       k_norm_step<<<1, 1, 0, s>>>(W.h, W.T, ncv, j, W.scal);
       count_launch();
+      if (j >= 0) {  // the same seed on every replica: they stay identical
+        k_refill<<<1, 1024, 0, s>>>(W.V, ld, cnt, N, 0x5EEDull + 1 + (uint64_t)ops, rep[g].wv, W.h, W.scal);
+        count_launch();
+      }
     }
     return BSG_OK;
   };
@@ -621,13 +688,11 @@ int lanczos_svd(std::vector<SvdShard> &sh, const int *ind_row, int nr, int ncol_
     int nkeep = k + std::min(nconv, (ncv - k) / 2);
     if (nkeep == 1 && ncv > 3) nkeep = ncv / 2;
     nkeep = std::min(nkeep, ncv - 1);
+    // the kept block of T is diag(theta); its arrowhead (column nkeep, b_i = beta * last row of the Ritz vectors) is not
+    // written: the next step computes that column as Gram-Schmidt coefficients <y_i, A v_nkeep> (k_tcol), which
+    // supersede the recurrence's b_i in both the device copy and the host readback
     std::fill(T.begin(), T.end(), 0.0);
-    for (int i = 0; i < nkeep; i++) {
-      T[(size_t)i * ncv + i] = theta[i];
-      double b = beta_last * Sm[(size_t)i * ncv + (ncv - 1)];
-      T[(size_t)nkeep * ncv + i] = b;
-      T[(size_t)i * ncv + nkeep] = b;
-    }
+    for (int i = 0; i < nkeep; i++) T[(size_t)i * ncv + i] = theta[i];
     for (int g = 0; g < G; g++) {
       BSG_TRY(bind_device(sh[g].h));
       SvdWork &W = rep[g].W;
