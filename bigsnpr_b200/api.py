@@ -1413,6 +1413,143 @@ def snp_ldpred2_inf(corr, df_beta, h2):
     return beta_inf * scale
 
 
+# ---- LDpred2-auto -------------------------------------------------------------------------------------------------------
+
+_MRG_M1, _MRG_M2 = 4294967087, 4294944443
+
+
+def _mrg_matpow(A, e, m):
+    """A^e mod m for a 3 x 3 matrix of Python ints."""
+    R = [[int(i == j) for j in range(3)] for i in range(3)]
+    while e:
+        if e & 1:
+            R = [[sum(R[i][k] * A[k][j] for k in range(3)) % m for j in range(3)] for i in range(3)]
+        A = [[sum(A[i][k] * A[k][j] for k in range(3)) % m for j in range(3)] for i in range(3)]
+        e >>= 1
+    return R
+
+
+_MRG_A1 = [[0, 1, 0], [0, 0, 1], [_MRG_M1 - 810728, 1403580, 0]]
+_MRG_A2 = [[0, 1, 0], [0, 0, 1], [_MRG_M2 - 1370589, 0, 527612]]
+_MRG_J1, _MRG_J2 = _mrg_matpow(_MRG_A1, 2 ** 127, _MRG_M1), _mrg_matpow(_MRG_A2, 2 ** 127, _MRG_M2)
+
+
+def mrg32k3a_next_stream(state):
+    """The MRG32k3a state 2^127 draws further (parallel::nextRNGStream): the start of the next stream."""
+    s = [int(v) for v in state]
+    a = [sum(_MRG_J1[i][k] * s[k] for k in range(3)) % _MRG_M1 for i in range(3)]
+    b = [sum(_MRG_J2[i][k] * s[3 + k] for k in range(3)) % _MRG_M2 for i in range(3)]
+    return np.array(a + b, dtype=np.uint32)
+
+
+def mrg32k3a_seed(seed):
+    """The first MRG32k3a state of `seed` (an integer taken mod 2^32): x <- 69069 x + 1 (mod 2^32) applied 50 times, then
+    once more for each of the six words, again while the word is not below m2."""
+    x = int(seed) & 0xFFFFFFFF
+    for _ in range(50):
+        x = (69069 * x + 1) & 0xFFFFFFFF
+    out = []
+    for _ in range(6):
+        x = (69069 * x + 1) & 0xFFFFFFFF
+        while x >= _MRG_M2:
+            x = (69069 * x + 1) & 0xFFFFFFFF
+        out.append(x)
+    return np.array(out, dtype=np.uint32)
+
+
+def _ldpred2_auto_call(corr, beta_hat, n_vec, log_var, ind_sub, p_init, h2_init, burn_in, num_iter, report_step,
+                       no_jump_sign, shrink_corr, use_mle, p_bounds, alpha_bounds, mean_ld, rng_state, sample=True):
+    """bsg_ldpred2_auto: a dict of the m x nchain estimates, the (burn_in + num_iter) x nchain paths, the dense
+    m x n_reports x nchain sample_beta (None unless `sample`) and each chain's device seconds."""
+    m, nchain = int(np.size(beta_hat)), int(np.size(p_init))
+    T, nrep = int(burn_in) + int(num_iter), int(num_iter) // max(int(report_step), 1)
+    rng = np.ascontiguousarray(np.asarray(rng_state, dtype=np.uint32).reshape(nchain * 6))
+    est = [np.empty((m, nchain), order="F") for _ in range(3)]
+    paths = [np.empty((T, nchain), order="F") for _ in range(3)]
+    smp = np.empty((m, nrep, nchain), order="F") if sample else None
+    secs = np.empty(nchain)
+    check(lib().bsg_ldpred2_auto(
+        corr._h, _pd(_f64(beta_hat)), _pd(_f64(n_vec)), _pd(_f64(log_var)), m, _pi(_i32(ind_sub)), nchain,
+        _pd(_f64(p_init)), float(h2_init), int(burn_in), int(num_iter), int(report_step), int(bool(no_jump_sign)),
+        float(shrink_corr), int(bool(use_mle)), _pd(_f64(p_bounds)), _pd(_f64(alpha_bounds)), float(mean_ld),
+        rng.ctypes.data_as(C.POINTER(C.c_uint)), *(_pd(a) for a in est), *(_pd(a) for a in paths),
+        None if smp is None else _pd(smp), _pd(secs)))
+    out = dict(zip(("beta_est", "postp_est", "corr_est"), est))
+    out.update(zip(("path_p_est", "path_h2_est", "path_alpha_est"), paths))
+    out["sample_beta"], out["time"] = smp, secs
+    return out
+
+
+def snp_ldpred2_auto(corr, df_beta, h2_init, vec_p_init=0.1, burn_in=500, num_iter=200, sparse=False, verbose=False,
+                     report_step=None, allow_jump_sign=True, shrink_corr=1, use_MLE=True, p_bounds=(1e-5, 1),
+                     alpha_bounds=(-1.5, 0.5), ind_corr=None, ncores=1, seed=None):
+    """R/LDpred2.R:203-286: LDpred2-auto, every chain (one per vec_p_init) in one bsg_ldpred2_auto launch.
+
+    corr: an SFBM; df_beta: a mapping with beta, beta_se and n_eff; ind_corr: 1-based columns of corr, one per row of
+    df_beta (default all); report_step None is num_iter + 1.  Returns a list over vec_p_init (in its order) of dicts with
+    beta_est (allele scale), postp_est, corr_est, sample_beta (scipy.sparse.csc_matrix, one row per row of df_beta as in
+    the reference, num_iter // report_step columns, not on the allele scale), path_p_est, path_h2_est, path_alpha_est, h2_est, p_est, alpha_est,
+    h2_init, p_init.
+
+    The chains run in R's order(-vec_p_init) (large p first, ties in input order); the i-th of that order draws from the
+    MRG32k3a stream mrg32k3a_seed(seed) jumped i x 2^127 draws (parallel::nextRNGStream's jump).  seed None takes one from
+    NumPy's global generator.  The draws follow R's sampler but are not R's stream: see DESIGN.md §4.15.  The MLE step
+    returns the minimiser of the reference's objective over its box, where R returns the point L-BFGS-B stops at.
+    sparse=True (ldpred2_gibbs_one, the grid model's sampler) is not implemented."""
+    if sparse:
+        raise NotImplementedError("sparse = TRUE needs ldpred2_gibbs_one (the grid model's sampler), not implemented.")
+    if not hasattr(df_beta, "__getitem__") or not hasattr(df_beta, "__contains__"):
+        raise TypeError("'df_beta' is not of class 'data.frame'.")
+    beta, beta_se, n_eff = (_df_column(df_beta, k) for k in ("beta", "beta_se", "n_eff"))
+    if not isinstance(corr, SFBM):
+        raise TypeError("'corr' is not of class 'SFBM'.")
+    ind_corr = corr.cols_along() if ind_corr is None else _i32(ind_corr)
+    _assert_lengths(ind_corr, beta)
+    if np.any((ind_corr < 1) | (ind_corr > corr.ncol)):
+        raise ValueError("all(ind.corr %in% cols_along(corr)) is not TRUE")
+    if not np.all(beta_se > 0):
+        raise ValueError("'df_beta$beta_se' should have only positive values.")
+    h2_init = float(h2_init)
+    if not h2_init > 0:
+        raise ValueError("'h2_init' should have only positive values.")
+    num_iter, burn_in = int(num_iter), int(burn_in)
+    report_step = num_iter + 1 if report_step is None else int(report_step)
+    vec_p_init = _f64(np.asarray(vec_p_init, dtype=np.float64).reshape(-1))
+    N = n_eff
+    sd = 1 / np.sqrt(N * beta_se ** 2 + beta ** 2)
+    beta_hat = beta * sd
+    ind_sub = _i32(ind_corr - 1)
+    mean_ld = float(np.mean(ld_scores_sfbm(corr, ind_corr)))
+    ord_ = np.argsort(-vec_p_init, kind="stable")
+    if seed is None:
+        seed = int(np.random.randint(0, 2 ** 31 - 1))
+    st = mrg32k3a_seed(seed)
+    states = []
+    for _ in range(ord_.size):
+        states.append(st)
+        st = mrg32k3a_next_stream(st)
+    r = _ldpred2_auto_call(corr, beta_hat, N, 2 * np.log(sd), ind_sub, vec_p_init[ord_], h2_init, burn_in, num_iter,
+                           report_step, not allow_jump_sign, shrink_corr, use_MLE, np.asarray(p_bounds, dtype=np.float64),
+                           np.asarray(alpha_bounds, dtype=np.float64) + 1, mean_ld, np.array(states), sample=True)
+    import scipy.sparse as sp
+
+    res = [None] * ord_.size
+    for i, c in enumerate(ord_):
+        out = {"beta_est": r["beta_est"][:, i] / sd, "postp_est": r["postp_est"][:, i].copy(),
+               "corr_est": r["corr_est"][:, i].copy()}
+        out["sample_beta"] = sp.csc_matrix(r["sample_beta"][:, :, i])
+        for k in ("path_p_est", "path_h2_est", "path_alpha_est"):
+            out[k] = r[k][:, i].copy()
+        tail = slice(out["path_h2_est"].size - num_iter, None)
+        out["h2_est"] = float(np.mean(out["path_h2_est"][tail]))
+        out["p_est"] = float(np.mean(out["path_p_est"][tail]))
+        out["alpha_est"] = float(np.mean(out["path_alpha_est"][tail]))
+        out["h2_init"], out["p_init"] = h2_init, float(vec_p_init[c])
+        out["time"] = float(r["time"][i])
+        res[c] = out
+    return res
+
+
 def _wlm(x, y, w):
     """R/ldsc.R:11-22 (stats::lm.wfit(cbind(1, x), y, w)), in its formula order."""
     wx = w * x

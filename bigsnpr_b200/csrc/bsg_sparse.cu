@@ -23,13 +23,19 @@
 // No FMA contraction (__dadd_rn / __dsub_rn / __dmul_rn / __ddiv_rn).  One iteration is four launches (t = A p + d o p;
 // chunk sums of p.t; alpha, x, r and chunk sums of r.r; the stopping test and p); a done flag in device memory turns the
 // rest of a block of CG_BLOCK enqueued iterations into no-ops, and the host reads it once per block.
+//
+// LDpred2-auto (src/ldpred2-auto.cpp:56-202): one CTA per chain, lassosum2's scan over a seeded MRG32k3a stream per chain,
+// the arithmetic in bsg_ldpred2_auto.cuh (DESIGN.md §4.15).
 #include <float.h>
+#include <limits.h>
 #include <math.h>
 #include <string.h>
 
+#include <cmath>
 #include <vector>
 
 #include "bsg_internal.cuh"
+#include "bsg_ldpred2_auto.cuh"
 
 struct bsg_sfbm {
   int device = 0;
@@ -360,6 +366,243 @@ __global__ void __launch_bounds__(CG_DT) k_cg_direction(const double *__restrict
   if (lead) st->rn2 = rn2, st->ab[(it + 1) & 1] = rn2;
 }
 
+// ---- LDpred2-auto: one CTA per chain -------------------------------------------------------------------------------------
+
+struct LdaArgs {
+  const double *beta_hat, *n_vec, *log_var, *p_init;
+  const int *ind_sub;
+  const uint32_t *rng;  // 6 words per chain
+  int m, burn_in, num_iter, report_step, nrep, no_jump_sign, use_mle;
+  double h2_init, shrink, p_lo, p_hi, t_lo, t_hi, mean_ld, gap0;
+  // outputs, per chain: m (estimates), T = burn_in + num_iter (paths), m x nrep (sample, may be null)
+  double *beta_est, *postp_est, *corr_est, *path_p, *path_h2, *path_alpha, *sample;
+  // scratch, per chain: ncol (dot), m (the others)
+  double *dot, *cb, *avg_b, *avg_p, *avg_bh, *abuf, *bbuf;
+  int *causal;
+  unsigned long long *ns;
+};
+
+// Sum over k < nb of b_k exp(-t a_k) (b non-null) or of a_k, in one fixed order: thread i folds k = i, i + LT, ... from
+// 0, then the pairwise tree v[i] += v[i + w], w = LT / 2 .. 1.  Every thread returns the sum.
+__device__ double lda_red(const double *__restrict__ a, const double *__restrict__ b, double t, int nb, double *sh) {
+  const int tid = threadIdx.x;
+  double s = 0;
+  for (int k = tid; k < nb; k += LT) s = __dadd_rn(s, b ? __dmul_rn(b[k], lda_exp(__dmul_rn(-t, a[k]))) : a[k]);
+  sh[tid] = s;
+  __syncthreads();
+  for (int w = LT / 2; w >= 32; w >>= 1) {
+    if (tid < w) sh[tid] = s = __dadd_rn(s, sh[tid + w]);
+    __syncthreads();
+  }
+  if (tid < 32) {
+    for (int w = 16; w; w >>= 1) s = __dadd_rn(s, __shfl_down_sync(0xffffffffu, s, w));
+    if (tid == 0) sh[0] = s;
+  }
+  __syncthreads();
+  s = sh[0];
+  __syncthreads();
+  return s;
+}
+
+__global__ void __launch_bounds__(LT) k_ldpred2_auto(const long long *__restrict__ p, const int *__restrict__ rows,
+                                                     const int *__restrict__ first_i, const double *__restrict__ x, int ncol,
+                                                     const LdaArgs A) {
+  __shared__ lda_mat s_pw[32];  // A^(2^i)
+  __shared__ lda_mat s_ln[32];  // A^(l + 1): lane l's draw is row 2 of it applied to the state
+  __shared__ lda_mat s_adv;     // A^(LT - 1): a bootstrap thread's stride
+  __shared__ double s_red[LT];
+  __shared__ uint32_t s_rng[6];
+  __shared__ int s_cmd, s_nb;
+  __shared__ double s_shift, s_p, s_h2, s_par[2], s_cur_h2;
+  const int c = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const unsigned long long t0 = globaltimer();
+  const int m = A.m, T = A.burn_in + A.num_iter;
+  double *dp = A.dot + (size_t)c * ncol, *cb = A.cb + (size_t)c * m;
+  double *avg_b = A.avg_b + (size_t)c * m, *avg_p = A.avg_p + (size_t)c * m, *avg_bh = A.avg_bh + (size_t)c * m;
+  double *abuf = A.abuf + (size_t)c * m, *bbuf = A.bbuf + (size_t)c * m;
+  int *causal = A.causal + (size_t)c * m;
+  double *path_p = A.path_p + (size_t)c * T, *path_h2 = A.path_h2 + (size_t)c * T, *path_alpha = A.path_alpha + (size_t)c * T;
+  double *sample = A.sample ? A.sample + (size_t)c * m * A.nrep : nullptr;
+  if (tid == 0) lda_pow2_table(s_pw, 32);
+  for (int i = tid; i < ncol; i += LT) dp[i] = 0;
+  for (int i = tid; i < m; i += LT) cb[i] = 0, avg_b[i] = 0, avg_p[i] = 0, avg_bh[i] = 0;
+  for (int i = tid; i < T; i += LT) path_p[i] = na_real(), path_h2[i] = na_real(), path_alpha[i] = na_real();
+  if (sample)
+    for (size_t i = tid; i < (size_t)m * A.nrep; i += LT) sample[i] = 0;
+  __syncthreads();
+  if (tid < 32) s_ln[tid] = lda_mat_pow(s_pw, tid + 1);
+  if (tid == 32) s_adv = lda_mat_pow(s_pw, LT - 1);
+  if (tid == 0) {  // src/ldpred2-auto.cpp:91-94
+    for (int i = 0; i < 6; i++) s_rng[i] = A.rng[6 * c + i];
+    const double h2 = A.h2_init < 1e-3 ? 1e-3 : A.h2_init;
+    double pp = A.p_lo < A.p_init[c] ? A.p_init[c] : A.p_lo;
+    pp = A.p_hi < pp ? A.p_hi : pp;
+    s_p = pp, s_h2 = h2, s_cur_h2 = 0;
+    s_par[0] = 0, s_par[1] = __ddiv_rn(h2, __dmul_rn((double)m, pp));
+  }
+  __syncthreads();
+  int next_k = A.burn_in + A.report_step - 1, irep = 0;
+  // warp 0's sweep state (every lane holds the same values)
+  uint32_t st[6];
+  double gap = 0, cur_h2 = 0;
+  int nb = 0;
+  for (int k = 0; k < T; k++) {
+    if (warp == 0) {
+      for (int i = 0; i < 6; i++) st[i] = s_rng[i];
+      cur_h2 = s_cur_h2, gap = 0, nb = 0;
+    }
+    const double inv_odd_p = __ddiv_rn(__dsub_rn(1.0, s_p), s_p), apo = s_par[0], sigma2 = s_par[1];
+    int j = 0;
+    for (;;) {
+      if (warp == 0) {
+        int cmd = CMD_NEXT_SWEEP;
+        double shift = 0;
+        while (j < m) {
+          const int jj = j + lane, nv = min(32, m - j);
+          const bool valid = jj < m;
+          lda_coord_t co = {0, 0, 0, 0};
+          double cur = 0;
+          int j2 = 0;
+          bool sel = false;
+          if (valid) {
+            j2 = A.ind_sub[jj];
+            cur = cb[jj];
+            co = lda_coord(A.beta_hat[jj], dp[j2], cur, A.n_vec[jj], A.log_var[jj], A.shrink, A.use_mle, apo, sigma2,
+                           inv_odd_p);
+            // the draw lane positions after the state: row 2 of A^(lane + 1) in each component
+            const uint32_t p1 = lda_mulmod3(s_ln[lane].a + 6, st, LDA_M1), p2 = lda_mulmod3(s_ln[lane].a + 15, st + 3, LDA_M2);
+            sel = co.postp > lda_u01(p1, p2);
+          }
+          // the first lane that draws a normal or changes beta; the lanes before it consume one uniform each
+          const unsigned stop = __ballot_sync(0xffffffffu, valid && (sel || cur != 0));
+          const int last = stop ? __ffs(stop) - 1 : nv - 1;
+          if (valid && lane <= last && k >= A.burn_in) {
+            avg_p[jj] = __dadd_rn(avg_p[jj], co.postp);
+            avg_b[jj] = __dadd_rn(avg_b[jj], __dmul_rn(co.C3, co.postp));
+            avg_bh[jj] = __dadd_rn(avg_bh[jj], co.dps);
+          }
+          lda_mat_apply(&s_ln[last], st);
+          if (!stop) {
+            j += nv;
+            continue;
+          }
+          const bool lsel = __shfl_sync(0xffffffffu, sel, last);
+          const double lcur = __shfl_sync(0xffffffffu, cur, last), C3 = __shfl_sync(0xffffffffu, co.C3, last);
+          const double C4 = __shfl_sync(0xffffffffu, co.C4, last), dps = __shfl_sync(0xffffffffu, co.dps, last);
+          const int lj2 = __shfl_sync(0xffffffffu, j2, last);
+          double diff = -lcur, nbeta = 0;
+          if (lsel) {  // src/ldpred2-auto.cpp:134-150
+            const double samp = lda_rnorm(C3, __dsqrt_rn(C4), st);
+            if (!(A.no_jump_sign && __dmul_rn(samp, lcur) < 0)) {
+              nbeta = samp;
+              diff = __dadd_rn(diff, samp);
+              if (lane == 0) causal[nb] = j + last;
+              nb++;
+              gap = __dadd_rn(gap, __dmul_rn(samp, samp));
+            }
+          }
+          if (lane == 0) cb[j + last] = nbeta;
+          j += last + 1;
+          if (diff != 0) {
+            cur_h2 = __dadd_rn(cur_h2, __dmul_rn(diff, __dadd_rn(__dmul_rn(2.0, dps), diff)));
+            cmd = lj2;
+            shift = diff;
+            break;
+          }
+        }
+        if (lane == 0) {
+          s_cmd = cmd;
+          s_shift = shift;
+        }
+      }
+      __syncthreads();
+      const int cmd = s_cmd;
+      if (cmd < 0) break;
+      {  // sfbm->incr_mult_col(j2, dotprods, diff)
+        const double shift = s_shift;
+        const long long lo = p[cmd], up = p[cmd + 1];
+        if (rows) {
+          for (long long q = lo + tid; q < up; q += LT) {
+            const int i = rows[q];
+            dp[i] = __dadd_rn(dp[i], __dmul_rn(x[q], shift));
+          }
+        } else {
+          const int i0 = first_i[cmd];
+          for (long long q = lo + tid; q < up; q += LT) {
+            const int i = i0 + (int)(q - lo);
+            dp[i] = __dadd_rn(dp[i], __dmul_rn(x[q], shift));
+          }
+        }
+      }
+      __syncthreads();
+    }
+    if (tid == 0) {  // src/ldpred2-auto.cpp:161-168
+      s_cur_h2 = cur_h2, s_nb = nb;
+      if (gap > A.gap0) {
+        s_cmd = CMD_DIVERGED;
+      } else {
+        s_p = lda_draw_p(nb, m, A.mean_ld, A.p_lo, A.p_hi, st);
+        s_h2 = cur_h2 < 1e-3 ? 1e-3 : cur_h2;
+      }
+      for (int i = 0; i < 6; i++) s_rng[i] = st[i];
+    }
+    __syncthreads();
+    if (s_cmd == CMD_DIVERGED) {
+      for (int i = tid; i < m; i += LT) avg_b[i] = na_real(), avg_p[i] = na_real(), avg_bh[i] = na_real();
+      break;
+    }
+    const int nbc = s_nb;
+    if (A.use_mle) {
+      if (nbc > 0) {  // MLE_alpha(par_mle, ind_causal, log_var, curr_beta, alpha_bounds, boot = true)
+        uint32_t bs[6];
+        for (int i = 0; i < 6; i++) bs[i] = s_rng[i];
+        lda_skip(bs, tid, s_pw);
+        for (int kk = tid; kk < nbc; kk += LT) {  // draw kk of the bootstrap, by skip-ahead
+          const int jc = causal[(int)__dmul_rn((double)nbc, lda_unif(bs))];
+          abuf[kk] = A.log_var[jc];
+          bbuf[kk] = __dmul_rn(cb[jc], cb[jc]);
+          lda_mat_apply(&s_adv, bs);
+        }
+        __syncthreads();
+        if (tid == 0) lda_skip(s_rng, nbc, s_pw);
+        const double sum_a = lda_red(abuf, nullptr, 0, nbc, s_red);
+        const double s2_lo = __ddiv_rn(s_par[1], 2.0), s2_hi = __dmul_rn(s_par[1], 2.0);
+        lda_golden g;
+        double t = lda_golden_start(&g, A.t_lo, A.t_hi), s2;
+        for (;;) {
+          const double C = lda_red(abuf, bbuf, t, nbc, s_red);
+          if (!lda_golden_next(&g, lda_mle_profile(t, sum_a, C, nbc, s2_lo, s2_hi, &s2), &t)) break;
+        }
+        const double C = lda_red(abuf, bbuf, g.best_t, nbc, s_red);
+        lda_mle_profile(g.best_t, sum_a, C, nbc, s2_lo, s2_hi, &s2);
+        if (tid == 0) s_par[0] = g.best_t, s_par[1] = s2;
+      }
+    } else if (tid == 0) {
+      s_par[1] = __ddiv_rn(s_h2, __dmul_rn((double)m, s_p));
+    }
+    __syncthreads();
+    if (tid == 0) {
+      path_p[k] = s_p, path_h2[k] = s_h2;
+      if (A.use_mle) path_alpha[k] = __dsub_rn(s_par[0], 1.0);
+    }
+    if (k == next_k) {  // src/ldpred2-auto.cpp:185-191
+      if (sample)
+        for (int i = tid; i < nbc; i += LT) sample[causal[i] + (size_t)irep * m] = cb[causal[i]];
+      irep++;
+      next_k += A.report_step;
+    }
+    __syncthreads();
+  }
+  const double inv = (double)A.num_iter;
+  for (int i = tid; i < m; i += LT) {  // avg / num_iter, NA_real kept as it is
+    const double b = avg_b[i], q = avg_p[i], h = avg_bh[i];
+    A.beta_est[(size_t)c * m + i] = b != b ? b : __ddiv_rn(b, inv);
+    A.postp_est[(size_t)c * m + i] = q != q ? q : __ddiv_rn(q, inv);
+    A.corr_est[(size_t)c * m + i] = h != h ? h : __ddiv_rn(h, inv);
+  }
+  if (tid == 0 && A.ns) A.ns[c] = globaltimer() - t0;
+}
+
 static int bind(const bsg_sfbm *s) {
   BSG_CUDA(cudaSetDevice(s->device));
   return BSG_OK;
@@ -624,5 +867,87 @@ int bsg_sfbm_solve(bsg_sfbm *A, const double *b, const double *add_to_diag, int 
 }
 
 double bsg_sfbm_last_solve_ms(const bsg_sfbm *A) { return A ? A->last_solve_ms : -1.0; }
+
+int bsg_ldpred2_auto(bsg_sfbm *corr, const double *beta_hat, const double *n_vec, const double *log_var, int m,
+                     const int *ind_sub, int nchain, const double *p_init, double h2_init, int burn_in, int num_iter,
+                     int report_step, int no_jump_sign, double shrink_corr, int use_mle, const double *p_bounds,
+                     const double *alpha_bounds, double mean_ld, const unsigned *rng_state, double *beta_est,
+                     double *postp_est, double *corr_est, double *path_p, double *path_h2, double *path_alpha,
+                     double *sample_beta, double *seconds) {
+  if (!corr || m < 1 || nchain < 0) return fail(BSG_ERR_ARG, "null argument, m < 1 or nchain < 0");
+  if (!beta_hat || !n_vec || !log_var || !ind_sub || !p_bounds || !alpha_bounds)
+    return fail(BSG_ERR_ARG, "null argument");
+  if (nchain > 0 && (!p_init || !rng_state || !beta_est || !postp_est || !corr_est || !path_p || !path_h2 || !path_alpha))
+    return fail(BSG_ERR_ARG, "null argument");
+  if (corr->nrow != corr->ncol) return fail(BSG_ERR_DIM, "Incompatibility between dimensions.");
+  if (burn_in < 0 || num_iter < 1 || report_step < 1 || (long long)burn_in + num_iter > INT_MAX)
+    return fail(BSG_ERR_ARG, "burn_in must be >= 0, num_iter and report_step >= 1.");
+  if (!(p_bounds[0] <= p_bounds[1]) || !(p_bounds[0] > 0))
+    return fail(BSG_ERR_ARG, "p_bounds must satisfy 0 < p_bounds[0] <= p_bounds[1].");
+  if (!(alpha_bounds[0] <= alpha_bounds[1]) || !std::isfinite(alpha_bounds[0]) || !std::isfinite(alpha_bounds[1]))
+    return fail(BSG_ERR_ARG, "alpha_bounds must be finite with alpha_bounds[0] <= alpha_bounds[1].");
+  if (!(mean_ld > 0)) return fail(BSG_ERR_ARG, "mean_ld must be positive.");
+  for (int c = 0; c < nchain; c++) {  // MRG32k3a: each component below its modulus and not all zero
+    const unsigned *s = rng_state + 6 * c;
+    if (s[0] >= LDA_M1 || s[1] >= LDA_M1 || s[2] >= LDA_M1 || s[3] >= LDA_M2 || s[4] >= LDA_M2 || s[5] >= LDA_M2 ||
+        (s[0] | s[1] | s[2]) == 0 || (s[3] | s[4] | s[5]) == 0)
+      return fail(BSG_ERR_ARG, "rng_state of chain %d is not a valid MRG32k3a state.", c);
+  }
+  BSG_TRY(check_sub(corr, ind_sub, m));
+  if (nchain == 0) return BSG_OK;
+  BSG_TRY(bind(corr));
+  double ss = 0;  // src/ldpred2-auto.cpp:96-97, folded in order
+  for (int j = 0; j < m; j++) ss = ss + beta_hat[j] * beta_hat[j];
+  const int T = burn_in + num_iter, nrep = num_iter / report_step;
+  const size_t mc = (size_t)m * nchain, tc = (size_t)T * nchain;
+  cudaStream_t st = corr->stream;
+  Bufs b;
+  LdaArgs A{};
+  A.m = m, A.burn_in = burn_in, A.num_iter = num_iter, A.report_step = report_step;
+  A.nrep = sample_beta ? nrep : 0;
+  A.no_jump_sign = no_jump_sign != 0, A.use_mle = use_mle != 0;
+  A.h2_init = h2_init, A.shrink = shrink_corr, A.p_lo = p_bounds[0], A.p_hi = p_bounds[1];
+  A.t_lo = alpha_bounds[0], A.t_hi = alpha_bounds[1], A.mean_ld = mean_ld, A.gap0 = 2 * ss;
+  double *d_bh = nullptr, *d_n = nullptr, *d_lv = nullptr, *d_pi = nullptr;
+  int *d_sub = nullptr;
+  uint32_t *d_rng = nullptr;
+  cudaError_t e = b.up(&d_bh, beta_hat, (size_t)m, st);
+  if (e == cudaSuccess) e = b.up(&d_n, n_vec, (size_t)m, st);
+  if (e == cudaSuccess) e = b.up(&d_lv, log_var, (size_t)m, st);
+  if (e == cudaSuccess) e = b.up(&d_pi, p_init, (size_t)nchain, st);
+  if (e == cudaSuccess) e = b.up(&d_sub, ind_sub, (size_t)m, st);
+  if (e == cudaSuccess) e = b.up(&d_rng, (const uint32_t *)rng_state, (size_t)6 * nchain, st);
+  double **outs[] = {&A.beta_est, &A.postp_est, &A.corr_est, &A.cb, &A.avg_b, &A.avg_p, &A.avg_bh, &A.abuf, &A.bbuf};
+  for (double **o : outs)
+    if (e == cudaSuccess) e = b.alloc(o, mc);
+  double **paths[] = {&A.path_p, &A.path_h2, &A.path_alpha};
+  for (double **o : paths)
+    if (e == cudaSuccess) e = b.alloc(o, tc);
+  if (e == cudaSuccess) e = b.alloc(&A.dot, (size_t)corr->ncol * nchain);
+  if (e == cudaSuccess) e = b.alloc(&A.causal, mc);
+  if (e == cudaSuccess && A.nrep) e = b.alloc(&A.sample, mc * A.nrep);
+  if (e == cudaSuccess) e = b.alloc(&A.ns, (size_t)nchain);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    return fail(e == cudaErrorMemoryAllocation ? BSG_ERR_ALLOC : BSG_ERR_CUDA, "ldpred2_auto state (%s)", cudaGetErrorString(e));
+  }
+  A.beta_hat = d_bh, A.n_vec = d_n, A.log_var = d_lv, A.p_init = d_pi, A.ind_sub = d_sub, A.rng = d_rng;
+  k_ldpred2_auto<<<nchain, LT, 0, st>>>(corr->p, corr->rows, corr->first_i, corr->x, corr->ncol, A);
+  count_launch();
+  BSG_CUDA(cudaGetLastError());
+  BSG_CUDA(cudaMemcpyAsync(beta_est, A.beta_est, mc * sizeof(double), cudaMemcpyDeviceToHost, st));
+  BSG_CUDA(cudaMemcpyAsync(postp_est, A.postp_est, mc * sizeof(double), cudaMemcpyDeviceToHost, st));
+  BSG_CUDA(cudaMemcpyAsync(corr_est, A.corr_est, mc * sizeof(double), cudaMemcpyDeviceToHost, st));
+  BSG_CUDA(cudaMemcpyAsync(path_p, A.path_p, tc * sizeof(double), cudaMemcpyDeviceToHost, st));
+  BSG_CUDA(cudaMemcpyAsync(path_h2, A.path_h2, tc * sizeof(double), cudaMemcpyDeviceToHost, st));
+  BSG_CUDA(cudaMemcpyAsync(path_alpha, A.path_alpha, tc * sizeof(double), cudaMemcpyDeviceToHost, st));
+  if (A.nrep) BSG_CUDA(cudaMemcpyAsync(sample_beta, A.sample, mc * A.nrep * sizeof(double), cudaMemcpyDeviceToHost, st));
+  std::vector<unsigned long long> ns(nchain);
+  BSG_CUDA(cudaMemcpyAsync(ns.data(), A.ns, (size_t)nchain * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+  BSG_CUDA(cudaStreamSynchronize(st));
+  if (seconds)
+    for (int c = 0; c < nchain; c++) seconds[c] = ns[c] * 1e-9;
+  return BSG_OK;
+}
 
 }  // extern "C"

@@ -288,6 +288,28 @@ int bsg_sfbm_solve(bsg_sfbm *A, const double *b, const double *add_to_diag, int 
 /* device time in ms (CUDA events) of the iterations of the last bsg_sfbm_solve on this handle, no-op launches after
  * convergence included; 0 when it ran none */
 double bsg_sfbm_last_solve_ms(const bsg_sfbm *A);
+/* LDpred2-auto: src/ldpred2-auto.cpp:56-202 (ldpred2_gibbs_auto) for nchain chains in one launch, one CTA per chain.
+ * beta_hat, n_vec, log_var: m values (R/LDpred2.R:238-255 passes beta * sd, n_eff and 2 log sd); ind_sub: m 0-based
+ * columns of corr, any order, repeats allowed (BSG_ERR_BOUNDS out of range).  Chain c starts from p_init[c] and draws
+ * from the MRG32k3a state rng_state[6 c .. 6 c + 5] (as R's .Random.seed[2:7] for L'Ecuyer-CMRG, as unsigned words);
+ * p_bounds[2], alpha_bounds[2] (alpha + 1, as the .Call receives them), mean_ld as the .Call takes them.  The draws are
+ * the ones of DESIGN.md §4.15 (one uniform per coordinate, a normal when it is selected, rbeta, then the bootstrap), and
+ * the MLE step returns the minimiser of MLE_alpha's objective over its box (golden-section search in alpha + 1 over
+ * the objective profiled in sigma2), where the reference returns the point L-BFGS-B stops at.  Every output of a chain
+ * depends only on the inputs and its own state: bit-identical to the sequential CPU restatement.
+ * Outputs, column-major with one column per chain: beta_est, postp_est, corr_est (m x nchain: the averages over the
+ * num_iter sweeps after burn_in, divided by num_iter; NA_real on divergence); path_p, path_h2, path_alpha ((burn_in +
+ * num_iter) x nchain, NA_real past a divergence, and path_alpha all NA_real without use_mle); sample_beta (NULL allowed)
+ * m x (num_iter / report_step) x nchain, dense, the causal effects at every report_step-th sweep after burn_in;
+ * seconds[nchain] (NULL allowed) the device time of each chain.  m < 1, burn_in < 0, num_iter < 1, report_step < 1,
+ * p_bounds not 0 < lo <= hi, alpha_bounds not finite lo <= hi, mean_ld <= 0, an invalid state or a null pointer:
+ * BSG_ERR_ARG; a non-square corr: BSG_ERR_DIM. */
+int bsg_ldpred2_auto(bsg_sfbm *corr, const double *beta_hat, const double *n_vec, const double *log_var, int m,
+                     const int *ind_sub, int nchain, const double *p_init, double h2_init, int burn_in, int num_iter,
+                     int report_step, int no_jump_sign, double shrink_corr, int use_mle, const double *p_bounds,
+                     const double *alpha_bounds, double mean_ld, const unsigned *rng_state, double *beta_est,
+                     double *postp_est, double *corr_est, double *path_p, double *path_h2, double *path_alpha,
+                     double *sample_beta, double *seconds);
 
 /* ---- near-independent LD blocks (snp_ldsplit, R/split-LD.R:99-138) -------------------------------------------------- */
 /* Matrix::tril(corr) staged to HBM once: m x m lower triangle in CSC, p[m + 1] (non-decreasing, p[0] = 0), rows i

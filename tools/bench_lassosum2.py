@@ -36,8 +36,8 @@ def gpu_info():
         return "unavailable (%s)" % e
 
 
-def simulated_sumstats(corr, m, seed):
-    """beta = R b + e / sqrt(N): the full symmetric R from the upper CSC, 0.5 % causal SNPs, n_eff 60-100 % of 50,000."""
+def simulated_sumstats(corr, m, seed, n_eff=50000):
+    """beta = R b + e / sqrt(N): the full symmetric R from the upper CSC, 0.5 % causal SNPs, N 60-100 % of n_eff."""
     import scipy.sparse as sp
 
     p, i, x = corr
@@ -47,7 +47,7 @@ def simulated_sumstats(corr, m, seed):
     causal = rng.choice(m, m // 200, replace=False)
     b[causal] = rng.normal(size=causal.size) * np.sqrt(0.3 / causal.size)
     Rb = U @ b + U.T @ b - U.diagonal() * b
-    N = np.round(50000 * rng.uniform(0.6, 1.0, m))
+    N = np.round(n_eff * rng.uniform(0.6, 1.0, m))
     se = 1 / np.sqrt(N)
     return {"beta": Rb + rng.normal(size=m) * se, "beta_se": se, "n_eff": N}
 
