@@ -22,6 +22,7 @@ and error behaviour, so the parity tests read like the reference's testthat file
     sp_solve_sym / snp_ldpred2_inf   bigsparser's conjugate-gradient solve, R/LDpred2.R:27-42
     snp_ldsc / snp_ldsc2   R/ldsc.R:1-224 (host NumPy; the LD scores of snp_ldsc2 come from ld_scores_sfbm)
     snp_PRS / snp_grid_PRS   R/PRS.R:36-76, R/SCT.R:201-246 (bsg_prs_grid: every keep set of a chromosome in one call)
+    big_univLinReg           bigstatsr's univLinReg5 + R glue (not vendored; bsg_univlinreg), result class MHTest
 
 Everything computes on the GPU through libbsgpu; there is no CPU path here (LD score regression, a few
 weighted least-squares fits on per-variant vectors, runs on the host).
@@ -1959,3 +1960,65 @@ def snp_grid_PRS(G, all_keep, betas, lpS, n_thr_lpS=50, grid_lpS_thr=None, ind_r
     res = out.view(GridPRS)
     res.lpS, res.grid_lpS_thr, res.betas, res.all_keep = lpS, thr, betas, all_keep
     return res
+
+
+class MHTest:
+    """big_univLinReg's result (bigstatsr's `mhtest` data frame): columns `estim`, `std_err`, `score` (in ind.col order),
+    `transfo` = abs (what snp_clumping ranks on) and `predict`.  `df` is the t distribution's degrees of freedom."""
+
+    def __init__(self, estim, std_err, score, df, transfo=np.abs):
+        self.estim, self.std_err, self.score, self.df, self.transfo = estim, std_err, score, df, transfo
+
+    def __getitem__(self, name):
+        return {"estim": self.estim, "std.err": self.std_err, "std_err": self.std_err, "score": self.score}[name]
+
+    def __len__(self):
+        return self.score.size
+
+    def predict(self, log10=True):
+        """log10 p-values of the two-sided t test: (log 2 + log pt(|score|, df, upper tail)) / log 10; 10^that when
+        log10 is False.  -predict() is snp_PRS's lpS."""
+        from scipy import stats
+
+        lp = (np.log(2) + stats.t.logsf(np.abs(self.score), self.df)) / np.log(10)
+        return lp if log10 else 10 ** lp
+
+
+def univlinreg_covar_basis(covar_train, n, thr_eigval=1e-4):
+    """The R glue of big_univLinReg: U = the left singular vectors of cbind(1, covar.train) whose singular values, scaled
+    by 1 / (sqrt(n) + sqrt(ncol) - 1), exceed thr_eigval (a duplicated column or a copy of the intercept drops out here)."""
+    cols = [np.ones(n)]
+    if covar_train is not None:
+        cv = np.asarray(covar_train, dtype=np.float64)
+        cols.append(cv.reshape(n, -1) if cv.ndim == 1 else cv)
+    Cm = np.column_stack(cols)
+    u, d, _ = np.linalg.svd(Cm, full_matrices=False)
+    keep = d / (np.sqrt(n) + np.sqrt(Cm.shape[1]) - 1) > thr_eigval
+    return np.asfortranarray(u[:, keep])
+
+
+def big_univLinReg(X, y_train, ind_train=..., ind_col=..., covar_train=None, thr_eigval=1e-4, ncores=1):
+    """bigstatsr's big_univLinReg on the device (bsg_univlinreg): the regression of y_train on [1, covar_train, X[, j]]
+    for every column j of ind_col, in one pass over the matrix per 64 digit slices.  The SVD of the covariates, the choice
+    of K and the degrees of freedom n - K - 1 run here in NumPy.  Returns an MHTest."""
+    _assert_bed(X)
+    ind_train = X.rows_along() if ind_train is ... else _i32(ind_train)
+    ind_col = X.cols_along() if ind_col is ... else _i32(ind_col)
+    y_train = _f64(y_train).reshape(-1)
+    _assert_lengths(y_train, ind_train)
+    n = ind_train.size
+    if covar_train is not None:
+        cv = np.asarray(covar_train, dtype=np.float64)
+        if cv.shape[0] != n:
+            raise ValueError(ERROR_DIM)
+    U = univlinreg_covar_basis(covar_train, n, thr_eigval)
+    K = U.shape[1]
+    estim, std_err = np.empty(ind_col.size), np.empty(ind_col.size)
+    check(lib().bsg_univlinreg(X._h, _pi(ind_train), n, _pi(ind_col), ind_col.size, _pd(_f64(U.T).reshape(-1)), K,
+                               _pd(y_train), _pd(estim), _pd(std_err)))
+    return MHTest(estim, std_err, estim / std_err, n - K - 1)
+
+
+def univlinreg_last_ms():
+    """Device time of the last big_univLinReg call (CUDA events), in ms."""
+    return lib().bsg_univlinreg_last_ms()

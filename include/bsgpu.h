@@ -251,6 +251,24 @@ int bsg_prs_grid(bsg_bed *h, const int *ind_row, int nr, int nsets, const int *s
 /* device time in ms (CUDA events) of the last bsg_prs_grid, quantisation to the gathered output, copies excluded */
 double bsg_prs_last_ms(void);
 
+/* big_univLinReg (bigstatsr's univLinReg5 and its R glue; bigstatsr is not vendored in the reference): linear regression of
+ * y on [C, X[ind_row, j]] for every selected column j, C = the covariates with the intercept.  U is nr x K column-major,
+ * orthonormal, spanning the intercept (the first K left singular vectors of cbind(1, covar.train) the glue keeps);
+ * y[nr] is y.train.  ind_row: 1-based, repeats allowed (a repeated row counts as often as it appears), NULL = all;
+ * ind_col: 1-based, repeats in any order, NULL = all.  estim / std_err (nc each, in ind_col order):
+ *   x2 = x - U U'x,  y2 = y - U U'y,  estim = x2'y2 / x2'x2,  std.err = sqrt((y2'y2 - estim x2'y2) / (nr - K - 1) / x2'x2),
+ * evaluated as x2'x2 = SSx_c - |U'x_c|^2 with SSx_c from exact integer sums of x and x^2 and x_c, y_c centred (DESIGN.md
+ * section 4.16).  The V = K + 1 products x'y_c, x'U are exact integer sums of the codes times fixed-point digits (y_c 61
+ * bits, U 30 bits) from one read of the matrix per group of at most 64 digit slices.  NaN for a column with an NA code
+ * on an ind_row row, a constant column, or x2'x2 <= 0.  Dosage tables (bsg_dosage_scale D > 0): the same sums over the
+ * value bytes D x code, divided by D once per sum; other FBM.code256 tables: BSG_ERR_TYPE.  K < 1, nr - K - 1 < 1, a
+ * non-finite y or U entry, or a U whose span misses the intercept: BSG_ERR_ARG; indices out of range: BSG_ERR_BOUNDS;
+ * scratch larger than the free device memory: BSG_ERR_ALLOC with the bytes needed, before any allocation. */
+int bsg_univlinreg(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, int nc, const double *U, int K,
+                   const double *y, double *estim, double *std_err);
+/* device time in ms (CUDA events) of the last bsg_univlinreg: vector upload to the statistics, copies back excluded */
+double bsg_univlinreg_last_ms(void);
+
 /* ---- sparse LD matrix (bigsparser's SFBM) and summary-statistics PRS -------------------------------------- */
 /* as_SFBM(corr[, compact]) staged to HBM once, in bigsparser's storage as bigsnpr reads it (src/ld-scores-sfbm.cpp:14-66):
  *   - p: ncol + 1 doubles, non-decreasing integers starting at 0 (X$p);
