@@ -23,6 +23,7 @@ and error behaviour, so the parity tests read like the reference's testthat file
     snp_ldsc / snp_ldsc2   R/ldsc.R:1-224 (host NumPy; the LD scores of snp_ldsc2 come from ld_scores_sfbm)
     snp_PRS / snp_grid_PRS   R/PRS.R:36-76, R/SCT.R:201-246 (bsg_prs_grid: every keep set of a chromosome in one call)
     big_univLinReg           bigstatsr's univLinReg5 + R glue (not vendored; bsg_univlinreg), result class MHTest
+    big_univLogReg           bigstatsr's IRLS + R glue (not vendored; bsg_univlogreg, glm.fit null model and refits here)
 
 Everything computes on the GPU through libbsgpu; there is no CPU path here (LD score regression, a few
 weighted least-squares fits on per-variant vectors, runs on the host).
@@ -1963,8 +1964,10 @@ def snp_grid_PRS(G, all_keep, betas, lpS, n_thr_lpS=50, grid_lpS_thr=None, ind_r
 
 
 class MHTest:
-    """big_univLinReg's result (bigstatsr's `mhtest` data frame): columns `estim`, `std_err`, `score` (in ind.col order),
-    `transfo` = abs (what snp_clumping ranks on) and `predict`.  `df` is the t distribution's degrees of freedom."""
+    """big_univLinReg's and big_univLogReg's result (bigstatsr's `mhtest` data frame): columns `estim`, `std_err`, `score`
+    (in ind.col order), `transfo` = abs (what snp_clumping ranks on) and `predict`.  `df` is the t distribution's degrees
+    of freedom; df = None means the normal distribution (big_univLogReg).  big_univLogReg also sets `niter` (IRLS steps,
+    or glm.fit iterations for a refitted SNP) and `refitted` (the SNPs whose IRLS did not meet tol in maxiter steps)."""
 
     def __init__(self, estim, std_err, score, df, transfo=np.abs):
         self.estim, self.std_err, self.score, self.df, self.transfo = estim, std_err, score, df, transfo
@@ -1976,11 +1979,12 @@ class MHTest:
         return self.score.size
 
     def predict(self, log10=True):
-        """log10 p-values of the two-sided t test: (log 2 + log pt(|score|, df, upper tail)) / log 10; 10^that when
-        log10 is False.  -predict() is snp_PRS's lpS."""
+        """log10 p-values of the two-sided test: (log 2 + log P(T > |score|)) / log 10 with T ~ t(df), or T ~ N(0, 1)
+        when df is None; 10^that when log10 is False.  -predict() is snp_PRS's lpS."""
         from scipy import stats
 
-        lp = (np.log(2) + stats.t.logsf(np.abs(self.score), self.df)) / np.log(10)
+        tail = stats.norm.logsf(np.abs(self.score)) if self.df is None else stats.t.logsf(np.abs(self.score), self.df)
+        lp = (np.log(2) + tail) / np.log(10)
         return lp if log10 else 10 ** lp
 
 
@@ -2022,3 +2026,98 @@ def big_univLinReg(X, y_train, ind_train=..., ind_col=..., covar_train=None, thr
 def univlinreg_last_ms():
     """Device time of the last big_univLinReg call (CUDA events), in ms."""
     return lib().bsg_univlinreg_last_ms()
+
+
+_GLM_THRESH, _GLM_MTHRESH = 30.0, -30.0  # R's binomial logit: make.link("logit") clamps eta beyond +-30
+_DBL_EPS = np.finfo(np.float64).eps
+
+
+def logit_glm_fit(A, y, eps=1e-8, maxit=25):
+    """R's glm.fit for family = binomial() (logit link, unit prior weights) on the design A (no intercept added):
+    mustart = (y + 0.5) / 2, iteratively reweighted least squares, converged when |dev - devold| / (|dev| + 0.1) < eps,
+    at most maxit iterations.  Returns (coefficients, standard errors from the last weighted fit, iterations, converged)."""
+    A, y = _f64(A), _f64(y)
+
+    def linkinv(eta):
+        t = np.where(eta < _GLM_MTHRESH, _DBL_EPS, np.where(eta > _GLM_THRESH, 1 / _DBL_EPS, np.exp(eta)))
+        return t / (1 + t)
+
+    def mu_eta(eta):
+        with np.errstate(over="ignore"):
+            e = np.exp(eta)
+            return np.where((eta > _GLM_THRESH) | (eta < _GLM_MTHRESH), _DBL_EPS, e / ((1 + e) * (1 + e)))
+
+    def deviance(mu):
+        with np.errstate(divide="ignore", invalid="ignore"):
+            return 2 * np.sum(np.where(y == 1, -np.log(mu), -np.log1p(-mu)))
+
+    mu = (y + 0.5) / 2
+    eta = np.log(mu / (1 - mu))
+    devold = deviance(mu)
+    coef, Aw, conv, it = np.zeros(A.shape[1]), A, False, 0
+    for it in range(1, maxit + 1):
+        me = mu_eta(eta)
+        z = eta + (y - mu) / me
+        w = np.sqrt(me * me / (mu * (1 - mu)))
+        Aw = A * w[:, None]
+        coef = np.linalg.lstsq(Aw, z * w, rcond=None)[0]
+        eta = A @ coef
+        mu = linkinv(eta)
+        dev = deviance(mu)
+        if abs(dev - devold) / (abs(dev) + 0.1) < eps:
+            conv = True
+            break
+        devold = dev
+    with np.errstate(invalid="ignore"):
+        se = np.sqrt(np.diag(np.linalg.pinv(Aw.T @ Aw)))
+    return coef, se, it, conv
+
+
+def _decode_column(X, ind_train, j):
+    """X[ind_train, j] as float64 (column j 1-based): the codes of a hard-call handle, byte / D of a dosage handle."""
+    if X.dosage_scale:
+        return bed_prodVec(X, np.ones(1), ind_train, _i32([j]))
+    return read_bed(X, ind_train, _i32([j]))[:, 0].astype(np.float64)
+
+
+def big_univLogReg(X, y01_train, ind_train=..., ind_col=..., covar_train=None, tol=1e-8, maxiter=20, ncores=1):
+    """bigstatsr's big_univLogReg on the device (bsg_univlogreg): the logistic regression of y01_train on
+    [1, covar_train, X[, j]] for every column j of ind_col, by per-SNP IRLS from the null model.  Here in NumPy: the basis
+    U of the covariates (univlinreg_covar_basis), the null model glm.fit(U, y01) and, for the SNPs whose IRLS did not meet
+    tol in maxiter steps, a glm.fit refit on [U, x] (same span as [1, covar, x], so the same estimate of x).  Returns an
+    MHTest with df = None (normal p-values), `niter` and `refitted`."""
+    _assert_bed(X)
+    ind_train = X.rows_along() if ind_train is ... else _i32(ind_train)
+    ind_col = X.cols_along() if ind_col is ... else _i32(ind_col)
+    y = _f64(y01_train).reshape(-1)
+    _assert_lengths(y, ind_train)
+    if not np.all((y == 0) | (y == 1)):
+        raise ValueError("'y01.train' should be composed of 0s and 1s.")
+    if y.size and (np.all(y == 0) or np.all(y == 1)):
+        raise ValueError("'y01.train' should have both 0s and 1s.")
+    n = ind_train.size
+    if covar_train is not None:
+        cv = np.asarray(covar_train, dtype=np.float64)
+        if cv.shape[0] != n:
+            raise ValueError(ERROR_DIM)
+    U = univlinreg_covar_basis(covar_train, n)
+    K = U.shape[1]
+    gamma0 = logit_glm_fit(U, y)[0]
+    m = ind_col.size
+    estim, std_err, niter = np.empty(m), np.empty(m), np.empty(m, dtype=np.int32)
+    check(lib().bsg_univlogreg(X._h, _pi(ind_train), n, _pi(ind_col), m, _pd(_f64(U.T).reshape(-1)), K, _pd(_f64(gamma0)),
+                               _pd(y), float(tol), int(maxiter), _pd(estim), _pd(std_err), _pi(niter)))
+    refitted = niter < 0
+    niter = np.abs(niter)
+    for c in np.flatnonzero(refitted):
+        x = _decode_column(X, ind_train, int(ind_col[c]))
+        coef, se, it, _ = logit_glm_fit(np.column_stack([U, x]), y)
+        estim[c], std_err[c], niter[c] = coef[-1], se[-1], it
+    res = MHTest(estim, std_err, estim / std_err, None)
+    res.niter, res.refitted = niter, refitted
+    return res
+
+
+def univlogreg_last_ms():
+    """Device time of the last big_univLogReg call's IRLS (CUDA events), in ms."""
+    return lib().bsg_univlogreg_last_ms()

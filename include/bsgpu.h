@@ -269,6 +269,28 @@ int bsg_univlinreg(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, i
 /* device time in ms (CUDA events) of the last bsg_univlinreg: vector upload to the statistics, copies back excluded */
 double bsg_univlinreg_last_ms(void);
 
+/* big_univLogReg's per-SNP IRLS (bigstatsr's IRLS; not vendored in the reference): logistic regression of y01 on
+ * A = [U, X[ind_row, j]] for every selected column j.  U is nr x K column-major (the orthonormal basis of cbind(1,
+ * covar.train) big_univLinReg's glue keeps; any finite basis is accepted), gamma0[K] the null model's coefficients on U
+ * (glm.fit of y01 on U), y01[nr] 0 / 1.  ind_row: 1-based, repeats allowed (each entry is one observation), NULL = all;
+ * ind_col: 1-based, repeats in any order, NULL = all.  Per SNP, from beta = (gamma0, 0):
+ *   eta = A beta, p = 1 / (1 + e^-eta), w = p (1 - p), H = A'WA, r = A'W z with W z = w eta + (y - p),
+ *   beta_new = H^-1 r, until max |beta_new - beta| < tol or maxiter steps.
+ * estim = beta_x, std_err = sqrt((H^-1)_xx) = 1 / L_xx of the last H solved (Cholesky, x last), niter = the steps taken,
+ * or -maxiter when tol was not met in maxiter steps (the caller refits those; estim / std_err then hold the last step).
+ * Every sum over observations runs in an order fixed by (nr, K) alone (DESIGN.md section 4.17): a SNP's bytes do not
+ * depend on the other columns of the call, their order or repeats.  NaN estim / std_err and niter = 0 for a column with an
+ * NA code on an ind_row row, a column constant over the rows, or an H whose factorisation meets a pivot <= 0 or a
+ * non-finite value.  Dosage tables (bsg_dosage_scale D > 0) read x = byte / D from the value copy; other FBM.code256
+ * tables: BSG_ERR_TYPE.  K < 1 or K > 80, nr < 1, tol <= 0, maxiter < 1, a y01 entry other than 0 / 1, non-finite U or
+ * gamma0: BSG_ERR_ARG; indices out of range: BSG_ERR_BOUNDS; scratch larger than the free device memory: BSG_ERR_ALLOC
+ * with the bytes needed, before any allocation. */
+int bsg_univlogreg(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, int nc, const double *U, int K,
+                   const double *gamma0, const double *y01, double tol, int maxiter, double *estim, double *std_err,
+                   int *niter);
+/* device time in ms (CUDA events) of the last bsg_univlogreg: column checks to the last IRLS step, copies excluded */
+double bsg_univlogreg_last_ms(void);
+
 /* ---- sparse LD matrix (bigsparser's SFBM) and summary-statistics PRS -------------------------------------- */
 /* as_SFBM(corr[, compact]) staged to HBM once, in bigsparser's storage as bigsnpr reads it (src/ld-scores-sfbm.cpp:14-66):
  *   - p: ncol + 1 doubles, non-decreasing integers starting at 0 (X$p);
