@@ -195,7 +195,9 @@ __global__ void k_cor_from_sums(const int *__restrict__ sums, const Tile *__rest
     }
     if (KIND == BAND_CLUMP) {
       const double cx = center[j0], cy = center[j];
-      const double r = (xySum - cy * xSum - cx * ySum + cx * cy * (double)nona) / (scale[j0] * scale[j]);
+      // the numerator's roundings spelled out (the three fused steps ptxas chose), so the flags cannot change with the compiler
+      const double num = __fma_rn(__dmul_rn(cx, cy), (double)nona, __fma_rn(cx, -ySum, __fma_rn(cy, -xSum, xySum)));
+      const double r = num / (scale[j0] * scale[j]);
       keep[o] = (r * r > thr_r2) ? 1 : 0;
       continue;
     }

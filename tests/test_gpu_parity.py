@@ -2,7 +2,8 @@
 on the same seeded inputs.  They mirror the reference's testthat files for this path (cited per test).
 
 Tolerances: bit-exact for counts / indices / decodes / correlations (integer sums + fp64 epilogue in the
-reference's operation order); matvecs agree with the oracle to 1e-11 relative to the vector scale (the
+reference's operation order; here on the fixtures, and in tests/test_gpu_cor.py across tile, batch and window edges
+against the exact model of tests/cor_ref.py); matvecs agree with the oracle to 1e-11 relative to the vector scale (the
 reference's own tests ask for 1.5e-8, north_star for 1e-6).  That tolerance is loose on purpose: it is the
 oracle's own rounding (one fp64 add per element) that it allows for.  The engine's accuracy is far tighter --
 |error| <= sum_t |g_t| 2^(-e-1) + a few ulps, about 2^-61 of max|v| sum|g| (2^-30 with two vectors per pass) --

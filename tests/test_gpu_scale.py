@@ -12,7 +12,7 @@ itself -- on the shapes whose code paths do not exist at fixture size:
 The relational form is the reference's own (tests/testthat/test-5-bed-prod-vec.R:18-41: products == dense decode %*% vector,
 default and random center / scale); the oracle's loops are that dense product restated literally.  Tolerances are the
 north_star's: bit-exact for counts / indices, 1e-6 relative for floating point -- the tests ask for much less
-(1e-11 of the vector scale for the products, 1e-10 for r, 1e-8 for K: 28-bit weights).
+(1e-11 of the vector scale for the products, 1e-8 for K: 28-bit weights); r is held to the oracle's bytes.
 """
 import numpy as np
 import pytest
@@ -117,8 +117,9 @@ def test_ksplit_shapes_vs_oracle(B, oracle, rng, shape, na_rate):
 @pytest.mark.parametrize("na_rate", [0.0, 0.005])
 def test_cfg3_slice_cor_ld_clumping_vs_oracle(B, oracle, na_rate):
     """configs[2]-shaped slice: 100,000 samples x 2,000 SNPs, 500-SNP window, LD-structured synthetic data (blocks of 50
-    correlated SNPs) so thresholds and pruning are exercised.  r is compared value by value with the same sparsity pattern,
-    LD scores to 1e-10, clumping indices exactly."""
+    correlated SNPs) so thresholds and pruning are exercised.  r is compared byte for byte with the same sparsity pattern,
+    LD scores to 1e-10 against the oracle (another summation order) and byte for byte against tests/cor_ref.py, clumping
+    indices exactly."""
     n, m = 100_000, 2_000
     kw = dict(seed=31, na_rate=na_rate, ld_rho=0.9, ld_block=50)
     o = oracle.synth_bed(n, m, **kw)
@@ -129,13 +130,16 @@ def test_cfg3_slice_cor_ld_clumping_vs_oracle(B, oracle, na_rate):
         p, i, x = B.bed_cor(g, size=500, thr_r2=thr_r2, infos_pos=pos)
         p0, i0, x0 = oracle.cor0(o, size=500, thr_r2=thr_r2, infos_pos=pos, ncores=nt)
         assert np.array_equal(p, p0) and np.array_equal(i, i0)
-        assert np.allclose(x, x0, rtol=0, atol=1e-12)
+        assert np.array_equal(x, x0, equal_nan=True)
         if thr_r2 > 0:
             assert 0 < x.size < 0.5 * m * 500  # the threshold really prunes on this data
     assert np.mean(np.abs(x) > 0.3) > 0.01
     ld = B.bed_ld_scores(g, size=500, infos_pos=pos)
     ld0 = oracle.ld0(o, size=500, infos_pos=pos, ncores=nt)
     assert np.max(np.abs(ld - ld0) / ld0) < 1e-10 and np.max(ld0) > 3
+    from tests import cor_ref
+
+    assert np.array_equal(ld, cor_ref.ld_scores(oracle.decode_dense(o), 500 * 1000.0, pos))  # k_ld_reduce's order, exactly
     # clumping on the first 500 SNPs, +-100 SNP window (the oracle's sweep is single-threaded by construction)
     sub = np.arange(1, 501, dtype=np.int32)
     excl = np.arange(501, m + 1)
@@ -205,7 +209,7 @@ def test_in_kernel_expansion_gram_tiles_vs_oracle(B, oracle, tmp_path):
         p0, i0, x0 = oracle.cor0(o, size=500, thr_r2=0.0, infos_pos=pos, ncores=nt)
         key = "cor_%g" % na
         assert np.array_equal(got[key + "_0"], p0) and np.array_equal(got[key + "_1"], i0)
-        assert np.allclose(got[key + "_2"], x0, rtol=0, atol=1e-12)
+        assert np.array_equal(got[key + "_2"], x0, equal_nan=True)
     for na in (0.0, 0.01):
         o = oracle.synth_bed(3_000, 10_000, seed=41, na_rate=na)
         K0 = oracle.bed_tcrossprodSelf(o, block_size=2000)[0]
