@@ -82,6 +82,12 @@ SIGNATURES = {
                                    C.c_int, C.c_int, C.c_int, C.c_double, C.c_int, c_dbl_p, c_dbl_p, C.c_double,
                                    C.POINTER(C.c_uint), c_dbl_p, c_dbl_p, c_dbl_p, c_dbl_p, c_dbl_p, c_dbl_p, c_dbl_p,
                                    c_dbl_p]),
+    "bsg_ldpred2_auto_ex": (C.c_int, [vp, c_dbl_p, c_dbl_p, c_dbl_p, C.c_int, c_int_p, C.c_int, c_dbl_p, C.c_double, C.c_int,
+                                      C.c_int, C.c_int, C.c_int, C.c_double, C.c_int, c_dbl_p, c_dbl_p, C.c_double,
+                                      C.POINTER(C.c_uint), c_dbl_p, c_dbl_p, c_dbl_p, c_dbl_p, c_dbl_p, c_dbl_p, c_dbl_p,
+                                      c_dbl_p, C.POINTER(C.c_uint)]),
+    "bsg_ldpred2_grid": (C.c_int, [vp, c_dbl_p, c_dbl_p, C.c_int, c_int_p, C.c_int, c_dbl_p, c_dbl_p, c_int_p, C.c_int,
+                                   C.c_int, C.c_int, C.POINTER(C.c_uint), c_dbl_p, c_dbl_p, c_dbl_p]),
     "bsg_ldcorr_open": (C.c_int, [C.c_int, c_i64_p, c_int_p, c_dbl_p, C.c_int, C.POINTER(vp)]),
     "bsg_ldcorr_close": (None, [vp]),
     "bsg_ldcorr_m": (C.c_int, [vp]),

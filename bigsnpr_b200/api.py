@@ -20,6 +20,7 @@ and error behaviour, so the parity tests read like the reference's testthat file
     as_SFBM / ld_scores_sfbm / snp_lassosum2   bigsparser's SFBM storage, src/ld-scores-sfbm.cpp:9-69, R/lassosum2.R:25-81
     snp_ldsplit / get_L / get_C   R/split-LD.R:3-40,99-138, src/split-LD.cpp:15-61,65-145,149-182
     sp_solve_sym / snp_ldpred2_inf   bigsparser's conjugate-gradient solve, R/LDpred2.R:27-42
+    snp_ldpred2_auto / snp_ldpred2_grid   R/LDpred2.R:203-286, R/LDpred2.R:73-140 (seeded MRG32k3a streams, DESIGN.md §4.15, §4.18)
     snp_ldsc / snp_ldsc2   R/ldsc.R:1-224 (host NumPy; the LD scores of snp_ldsc2 come from ld_scores_sfbm)
     snp_PRS / snp_grid_PRS   R/PRS.R:36-76, R/SCT.R:201-246 (bsg_prs_grid: every keep set of a chromosome in one call)
     big_univLinReg           bigstatsr's univLinReg5 + R glue (not vendored; bsg_univlinreg), result class MHTest
@@ -1301,13 +1302,13 @@ class Lassosum2Grid(np.ndarray):
     grid_param = None
 
 
-def _df_column(df, name):
+def _df_column(df, name, what="df_beta"):
     try:
         if name in df:
             return _f64(df[name])
     except TypeError:
         pass
-    raise ValueError("'df_beta' should have element '%s'." % name)
+    raise ValueError("'%s' should have element '%s'." % (what, name))
 
 
 def _lassosum2_grid(beta, beta_se, n_eff, delta, nlambda, lambda_min_ratio):
@@ -1460,9 +1461,11 @@ def mrg32k3a_seed(seed):
 
 
 def _ldpred2_auto_call(corr, beta_hat, n_vec, log_var, ind_sub, p_init, h2_init, burn_in, num_iter, report_step,
-                       no_jump_sign, shrink_corr, use_mle, p_bounds, alpha_bounds, mean_ld, rng_state, sample=True):
-    """bsg_ldpred2_auto: a dict of the m x nchain estimates, the (burn_in + num_iter) x nchain paths, the dense
-    m x n_reports x nchain sample_beta (None unless `sample`) and each chain's device seconds."""
+                       no_jump_sign, shrink_corr, use_mle, p_bounds, alpha_bounds, mean_ld, rng_state, sample=True,
+                       rng_out=False):
+    """bsg_ldpred2_auto_ex: a dict of the m x nchain estimates, the (burn_in + num_iter) x nchain paths, the dense
+    m x n_reports x nchain sample_beta (None unless `sample`), each chain's device seconds and, with `rng_out`, the
+    nchain x 6 MRG32k3a states the chains end in ("rng_out")."""
     m, nchain = int(np.size(beta_hat)), int(np.size(p_init))
     T, nrep = int(burn_in) + int(num_iter), int(num_iter) // max(int(report_step), 1)
     rng = np.ascontiguousarray(np.asarray(rng_state, dtype=np.uint32).reshape(nchain * 6))
@@ -1470,16 +1473,28 @@ def _ldpred2_auto_call(corr, beta_hat, n_vec, log_var, ind_sub, p_init, h2_init,
     paths = [np.empty((T, nchain), order="F") for _ in range(3)]
     smp = np.empty((m, nrep, nchain), order="F") if sample else None
     secs = np.empty(nchain)
-    check(lib().bsg_ldpred2_auto(
+    rout = np.empty((nchain, 6), dtype=np.uint32) if rng_out else None
+    check(lib().bsg_ldpred2_auto_ex(
         corr._h, _pd(_f64(beta_hat)), _pd(_f64(n_vec)), _pd(_f64(log_var)), m, _pi(_i32(ind_sub)), nchain,
         _pd(_f64(p_init)), float(h2_init), int(burn_in), int(num_iter), int(report_step), int(bool(no_jump_sign)),
         float(shrink_corr), int(bool(use_mle)), _pd(_f64(p_bounds)), _pd(_f64(alpha_bounds)), float(mean_ld),
         rng.ctypes.data_as(C.POINTER(C.c_uint)), *(_pd(a) for a in est), *(_pd(a) for a in paths),
-        None if smp is None else _pd(smp), _pd(secs)))
+        None if smp is None else _pd(smp), _pd(secs), None if rout is None else rout.ctypes.data_as(C.POINTER(C.c_uint))))
     out = dict(zip(("beta_est", "postp_est", "corr_est"), est))
     out.update(zip(("path_p_est", "path_h2_est", "path_alpha_est"), paths))
     out["sample_beta"], out["time"] = smp, secs
+    if rng_out:
+        out["rng_out"] = rout
     return out
+
+
+def _mrg_streams(seed, n):
+    """n MRG32k3a states: mrg32k3a_seed(seed), then each the previous jumped 2^127 draws (%dorng%'s streams)."""
+    st, out = mrg32k3a_seed(seed), []
+    for _ in range(n):
+        out.append(st)
+        st = mrg32k3a_next_stream(st)
+    return np.array(out, dtype=np.uint32).reshape(n, 6)
 
 
 def snp_ldpred2_auto(corr, df_beta, h2_init, vec_p_init=0.1, burn_in=500, num_iter=200, sparse=False, verbose=False,
@@ -1497,9 +1512,12 @@ def snp_ldpred2_auto(corr, df_beta, h2_init, vec_p_init=0.1, burn_in=500, num_it
     MRG32k3a stream mrg32k3a_seed(seed) jumped i x 2^127 draws (parallel::nextRNGStream's jump).  seed None takes one from
     NumPy's global generator.  The draws follow R's sampler but are not R's stream: see DESIGN.md §4.15.  The MLE step
     returns the minimiser of the reference's objective over its box, where R returns the point L-BFGS-B stops at.
-    sparse=True (ldpred2_gibbs_one, the grid model's sampler) is not implemented."""
+    sparse=True is not served here: snp_ldpred2_grid runs the same sparse sampler (ldpred2_gibbs_one) with a chain's
+    p_est and h2_est, on a stream of its own, and the C ABI's bsg_ldpred2_auto_ex / bsg_ldpred2_grid continue a chain's
+    own stream as R/LDpred2.R:266-279 does (DESIGN.md §4.15)."""
     if sparse:
-        raise NotImplementedError("sparse = TRUE needs ldpred2_gibbs_one (the grid model's sampler), not implemented.")
+        raise NotImplementedError("sparse = TRUE is not served by snp_ldpred2_auto; run snp_ldpred2_grid with the chains' "
+                                  "p_est and h2_est and sparse = TRUE.")
     if not hasattr(df_beta, "__getitem__") or not hasattr(df_beta, "__contains__"):
         raise TypeError("'df_beta' is not of class 'data.frame'.")
     beta, beta_se, n_eff = (_df_column(df_beta, k) for k in ("beta", "beta_se", "n_eff"))
@@ -1525,14 +1543,10 @@ def snp_ldpred2_auto(corr, df_beta, h2_init, vec_p_init=0.1, burn_in=500, num_it
     ord_ = np.argsort(-vec_p_init, kind="stable")
     if seed is None:
         seed = int(np.random.randint(0, 2 ** 31 - 1))
-    st = mrg32k3a_seed(seed)
-    states = []
-    for _ in range(ord_.size):
-        states.append(st)
-        st = mrg32k3a_next_stream(st)
     r = _ldpred2_auto_call(corr, beta_hat, N, 2 * np.log(sd), ind_sub, vec_p_init[ord_], h2_init, burn_in, num_iter,
                            report_step, not allow_jump_sign, shrink_corr, use_MLE, np.asarray(p_bounds, dtype=np.float64),
-                           np.asarray(alpha_bounds, dtype=np.float64) + 1, mean_ld, np.array(states), sample=True)
+                           np.asarray(alpha_bounds, dtype=np.float64) + 1, mean_ld, _mrg_streams(seed, ord_.size),
+                           sample=True)
     import scipy.sparse as sp
 
     res = [None] * ord_.size
@@ -1550,6 +1564,83 @@ def snp_ldpred2_auto(corr, df_beta, h2_init, vec_p_init=0.1, burn_in=500, num_it
         out["time"] = float(r["time"][i])
         res[c] = out
     return res
+
+
+def _ldpred2_grid_call(corr, beta_hat, n_vec, ind_sub, p, h2, sparse, burn_in, num_iter, rng_state, sampling=False):
+    """bsg_ldpred2_grid: a dict of the m x npoint beta_est (or, with `sampling`, the m x num_iter sample_beta of the one
+    point) and each point's device seconds ("time"); point g runs with p[g], h2[g], sparse[g] on the MRG32k3a state
+    rng_state[g]."""
+    p, h2 = _f64(np.asarray(p, dtype=np.float64).reshape(-1)), _f64(np.asarray(h2, dtype=np.float64).reshape(-1))
+    sparse = _i32(np.asarray(sparse).reshape(-1).astype(bool))
+    m, npoint = int(np.size(beta_hat)), p.size
+    rng = np.ascontiguousarray(np.asarray(rng_state, dtype=np.uint32).reshape(npoint * 6))
+    est = None if sampling else np.empty((m, npoint), order="F")
+    smp = np.empty((m, int(num_iter)), order="F") if sampling else None
+    secs = np.empty(npoint)
+    check(lib().bsg_ldpred2_grid(corr._h, _pd(_f64(beta_hat)), _pd(_f64(n_vec)), m, _pi(_i32(ind_sub)), npoint, _pd(p),
+                                 _pd(h2), _pi(sparse), int(burn_in), int(num_iter), int(bool(sampling)),
+                                 rng.ctypes.data_as(C.POINTER(C.c_uint)), None if est is None else _pd(est),
+                                 None if smp is None else _pd(smp), _pd(secs)))
+    return {"beta_est": est, "sample_beta": smp, "time": secs}
+
+
+def _ldpred2_grid_order(p, h2, sparse):
+    """R's order(-p, sparse, -h2): stable, large p first, then non-sparse first, then large h2 first."""
+    return np.lexsort((-np.asarray(h2, dtype=np.float64), np.asarray(sparse).astype(bool),
+                       -np.asarray(p, dtype=np.float64)))
+
+
+def snp_ldpred2_grid(corr, df_beta, grid_param, burn_in=50, num_iter=100, ncores=1, return_sampling_betas=False,
+                     ind_corr=None, seed=None):
+    """R/LDpred2.R:73-140: LDpred2-grid, every row of grid_param in one bsg_ldpred2_grid launch.
+
+    corr: an SFBM; df_beta: a mapping with beta, beta_se and n_eff; grid_param: a mapping with p, h2 and sparse (one
+    value per grid point); ind_corr: 1-based columns of corr, one per row of df_beta (default all).  Returns the m x
+    ngrid effects (one column per row of grid_param, in its order) times scale = sqrt(n_eff beta_se^2 + beta^2), a column
+    of NA where the point diverged; with return_sampling_betas (one row of grid_param only), the m x num_iter sampling
+    betas times scale.
+
+    The points run in R's order(-p, sparse, -h2) (stable); the i-th of that order draws from the MRG32k3a stream
+    mrg32k3a_seed(seed) jumped i x 2^127 draws, as snp_ldpred2_auto's chains do, and the sampling run from the first
+    stream.  seed None takes one from NumPy's global generator.  The draws follow R's sampler but are not R's stream: see
+    DESIGN.md §4.18."""
+    if not hasattr(df_beta, "__getitem__") or not hasattr(df_beta, "__contains__"):
+        raise TypeError("'df_beta' is not of class 'data.frame'.")
+    beta, beta_se, n_eff = (_df_column(df_beta, k) for k in ("beta", "beta_se", "n_eff"))
+    if not hasattr(grid_param, "__getitem__") or not hasattr(grid_param, "__contains__"):
+        raise TypeError("'grid_param' is not of class 'data.frame'.")
+    g_p, g_h2, g_sparse = (_df_column(grid_param, k, "grid_param") for k in ("p", "h2", "sparse"))
+    if not (g_p.size == g_h2.size == g_sparse.size):
+        raise ValueError(ERROR_DIM)
+    if not isinstance(corr, SFBM):
+        raise TypeError("'corr' is not of class 'SFBM'.")
+    ind_corr = corr.cols_along() if ind_corr is None else _i32(ind_corr)
+    _assert_lengths(ind_corr, beta)
+    if np.any((ind_corr < 1) | (ind_corr > corr.ncol)):
+        raise ValueError("all(ind.corr %in% cols_along(corr)) is not TRUE")
+    if not np.all(beta_se > 0):
+        raise ValueError("'df_beta$beta_se' should have only positive values.")
+    if not np.all(g_h2 > 0):
+        raise ValueError("'grid_param$h2' should have only positive values.")
+    N = n_eff
+    scale = np.sqrt(N * beta_se ** 2 + beta ** 2)
+    beta_hat = beta / scale
+    ind_sub = _i32(ind_corr - 1)
+    if seed is None:
+        seed = int(np.random.randint(0, 2 ** 31 - 1))
+    if return_sampling_betas:
+        if g_p.size != 1:
+            raise ValueError("Only one set of parameters is allowed when using 'return_sampling_betas'.")
+        r = _ldpred2_grid_call(corr, beta_hat, N, ind_sub, g_p, g_h2, g_sparse != 0, burn_in, num_iter,
+                               _mrg_streams(seed, 1), sampling=True)
+        return np.asfortranarray(r["sample_beta"] * scale[:, None])
+    ord_ = _ldpred2_grid_order(g_p, g_h2, g_sparse != 0)
+    r = _ldpred2_grid_call(corr, beta_hat, N, ind_sub, g_p[ord_], g_h2[ord_], g_sparse[ord_] != 0, burn_in, num_iter,
+                           _mrg_streams(seed, ord_.size))
+    beta_gibbs = np.empty_like(r["beta_est"])
+    beta_gibbs[:, ord_] = r["beta_est"]  # res_list[inv_ord]
+    with np.errstate(invalid="ignore"):  # a diverged point's NA column times scale
+        return np.asfortranarray(beta_gibbs * scale[:, None])
 
 
 def _wlm(x, y, w):

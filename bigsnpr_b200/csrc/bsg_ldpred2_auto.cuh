@@ -12,7 +12,9 @@
  *     (PPND16); rnorm(mu, sigma) = mu + sigma z, no draw when sigma == 0 or mu is not finite.
  *   - rbeta: Cheng's (1978) algorithms BB (min(a, b) > 1) and BC (otherwise), as R's rbeta uses them.
  *   - exp / log: Cody-Waite reduction and the minimax polynomials of fdlibm's e_exp.c / e_log.c (< 1 ulp).
- *   - the coordinate update of the Gibbs sweep, the MLE objective's profile in alpha + 1 and its golden-section search.
+ *   - the coordinate update of the Gibbs sweep, the MLE objective's profile in alpha + 1 and its golden-section search;
+ *   - LDpred2-grid's coordinate update (src/ldpred2.cpp:9-69, src/ldpred2-sampling.cpp:9-59) and the draw offset of a
+ *     warp lane when a sparse point skips the uniform of the coordinates it zeroes.
  */
 #ifndef BSG_LDPRED2_AUTO_CUH
 #define BSG_LDPRED2_AUTO_CUH
@@ -373,6 +375,42 @@ LDA_FN lda_coord_t lda_coord(double beta_hat, double dotprod, double cur, double
   o.postp = LDA_DIV(1.0, LDA_ADD(1.0, LDA_MUL(LDA_MUL(inv_odd_p, LDA_SQRT(LDA_ADD(1.0, C1))), e)));
   o.dps = LDA_ADD(LDA_MUL(shrink, dotprod), LDA_MUL(LDA_SUB(1.0, shrink), cur));
   return o;
+}
+
+/* One coordinate of LDpred2-grid's sweep (src/ldpred2.cpp:39-47, src/ldpred2-sampling.cpp:36-44) from its residual, in
+ * the reference's operation order.  The residual is formed by lda_grid_res: ldpred2_gibbs_one takes beta_hat - (dotprod -
+ * cur), ldpred2_gibbs_one_sampling (beta_hat + cur) - dotprod, two roundings of the same value. */
+typedef struct {
+  double postp, C3, C4;
+} lda_gcoord_t;
+
+LDA_FN double lda_grid_res(double beta_hat, double dotprod, double cur, int sampling) {
+  return sampling ? LDA_SUB(LDA_ADD(beta_hat, cur), dotprod) : LDA_SUB(beta_hat, LDA_SUB(dotprod, cur));
+}
+
+LDA_FN lda_gcoord_t lda_grid_coord(double res, double h2_per_var, double n, double inv_odd_p) {
+  lda_gcoord_t o;
+  const double C1 = LDA_MUL(h2_per_var, n);
+  const double C2 = LDA_DIV(1.0, LDA_ADD(1.0, LDA_DIV(1.0, C1)));
+  o.C3 = LDA_MUL(C2, res);
+  o.C4 = LDA_DIV(C2, n);
+  const double e = lda_exp(LDA_DIV(LDA_DIV(LDA_MUL(-o.C3, o.C3), o.C4), 2.0));
+  o.postp = LDA_DIV(1.0, LDA_ADD(1.0, LDA_MUL(LDA_MUL(inv_odd_p, LDA_SQRT(LDA_ADD(1.0, C1))), e)));
+  return o;
+}
+
+/* Whether the coordinate draws its uniform: a sparse point sets beta to 0 without a draw when postp < p */
+LDA_FN int lda_grid_draws(int sparse, double postp, double p) { return !(sparse && postp < p); }
+
+/* The draw offset of lane `lane` in a warp whose drawing lanes are the bits of `draws`: the number of uniforms the lanes
+ * below it take first.  Its uniform is the (offset + 1)-th from the warp's state, row 2 of A^(offset + 1). */
+LDA_FN int lda_grid_offset(uint32_t draws, int lane) {
+  const uint32_t below = draws & ((1u << lane) - 1u); /* lane < 32 */
+#ifdef __CUDA_ARCH__
+  return __popc(below);
+#else
+  return __builtin_popcount(below);
+#endif
 }
 
 /* p after a sweep with nb causal variants out of m (src/ldpred2-auto.cpp:166-168) */

@@ -26,6 +26,9 @@
 //
 // LDpred2-auto (src/ldpred2-auto.cpp:56-202): one CTA per chain, lassosum2's scan over a seeded MRG32k3a stream per chain,
 // the arithmetic in bsg_ldpred2_auto.cuh (DESIGN.md §4.15).
+//
+// LDpred2-grid (src/ldpred2.cpp:9-69, src/ldpred2-sampling.cpp:9-59): one CTA per grid point, the same scan, streams and
+// header; a sparse point's coordinates with postp < p take no uniform (DESIGN.md §4.18).
 #include <float.h>
 #include <limits.h>
 #include <math.h>
@@ -71,6 +74,29 @@ __device__ __forceinline__ double soft_thres(double z, double l1, double one_plu
   } else {
     const double num = __dadd_rn(z, l1);
     return (num < 0) ? __ddiv_rn(num, one_plus_l2) : 0;
+  }
+}
+
+// sfbm->incr_mult_col(j2, dotprods, shift) by the LT threads of a CTA, thread t from entry t: dp[i] += x_ij * shift over the
+// stored entries of column j2.  Each row of a column is stored once, so the updates do not collide.  t keeps the type the
+// kernel holds its thread index in (unsigned threadIdx.x or an int): ptxas allocates each kernel's registers as it did
+// when the loop was written inline, without spills.
+template <typename Tid>
+__device__ __forceinline__ void incr_mult_col(const long long *__restrict__ p, const int *__restrict__ rows,
+                                              const int *__restrict__ first_i, const double *__restrict__ x, int j2,
+                                              double shift, double *dp, Tid t) {
+  const long long lo = p[j2], up = p[j2 + 1];
+  if (rows) {
+    for (long long q = lo + t; q < up; q += LT) {
+      const int i = rows[q];
+      dp[i] = __dadd_rn(dp[i], __dmul_rn(x[q], shift));
+    }
+  } else {
+    const int i0 = first_i[j2];
+    for (long long q = lo + t; q < up; q += LT) {
+      const int i = i0 + (int)(q - lo);
+      dp[i] = __dadd_rn(dp[i], __dmul_rn(x[q], shift));
+    }
   }
 }
 
@@ -163,22 +189,7 @@ __global__ void __launch_bounds__(LT) k_lassosum2(const long long *__restrict__ 
           for (int i = threadIdx.x; i < m; i += LT) cb[i] = na_real();
         goto done;
       }
-      {  // sfbm->incr_mult_col(j2, dotprods, shift): each row of a column is stored once, so the updates do not collide
-        const double shift = s_shift;
-        const long long lo = p[cmd], up = p[cmd + 1];
-        if (rows) {
-          for (long long q = lo + threadIdx.x; q < up; q += LT) {
-            const int i = rows[q];
-            dp[i] = __dadd_rn(dp[i], __dmul_rn(x[q], shift));
-          }
-        } else {
-          const int i0 = first_i[cmd];
-          for (long long q = lo + threadIdx.x; q < up; q += LT) {
-            const int i = i0 + (int)(q - lo);
-            dp[i] = __dadd_rn(dp[i], __dmul_rn(x[q], shift));
-          }
-        }
-      }
+      incr_mult_col(p, rows, first_i, x, cmd, s_shift, dp, threadIdx.x);
       __syncthreads();
     }
     __syncthreads();  // s_cmd is rewritten by the next sweep
@@ -372,6 +383,7 @@ struct LdaArgs {
   const double *beta_hat, *n_vec, *log_var, *p_init;
   const int *ind_sub;
   const uint32_t *rng;  // 6 words per chain
+  uint32_t *rng_out;    // 6 words per chain, the state after the last sweep (may be null)
   int m, burn_in, num_iter, report_step, nrep, no_jump_sign, use_mle;
   double h2_init, shrink, p_lo, p_hi, t_lo, t_hi, mean_ld, gap0;
   // outputs, per chain: m (estimates), T = burn_in + num_iter (paths), m x nrep (sample, may be null)
@@ -518,22 +530,7 @@ __global__ void __launch_bounds__(LT) k_ldpred2_auto(const long long *__restrict
       __syncthreads();
       const int cmd = s_cmd;
       if (cmd < 0) break;
-      {  // sfbm->incr_mult_col(j2, dotprods, diff)
-        const double shift = s_shift;
-        const long long lo = p[cmd], up = p[cmd + 1];
-        if (rows) {
-          for (long long q = lo + tid; q < up; q += LT) {
-            const int i = rows[q];
-            dp[i] = __dadd_rn(dp[i], __dmul_rn(x[q], shift));
-          }
-        } else {
-          const int i0 = first_i[cmd];
-          for (long long q = lo + tid; q < up; q += LT) {
-            const int i = i0 + (int)(q - lo);
-            dp[i] = __dadd_rn(dp[i], __dmul_rn(x[q], shift));
-          }
-        }
-      }
+      incr_mult_col(p, rows, first_i, x, cmd, s_shift, dp, tid);
       __syncthreads();
     }
     if (tid == 0) {  // src/ldpred2-auto.cpp:161-168
@@ -600,11 +597,148 @@ __global__ void __launch_bounds__(LT) k_ldpred2_auto(const long long *__restrict
     A.postp_est[(size_t)c * m + i] = q != q ? q : __ddiv_rn(q, inv);
     A.corr_est[(size_t)c * m + i] = h != h ? h : __ddiv_rn(h, inv);
   }
+  if (tid == 0 && A.rng_out)
+    for (int i = 0; i < 6; i++) A.rng_out[6 * c + i] = s_rng[i];
   if (tid == 0 && A.ns) A.ns[c] = globaltimer() - t0;
+}
+
+// ---- LDpred2-grid: one CTA per grid point --------------------------------------------------------------------------------
+
+struct LdgArgs {
+  const double *beta_hat, *n_vec, *p, *h2;
+  const int *sparse, *ind_sub;
+  const uint32_t *rng;  // 6 words per point
+  int m, burn_in, num_iter;
+  double gap0;
+  double *beta_est, *sample;  // m per point; m x num_iter (SAMPLING, one point)
+  double *dot, *cb, *avg;     // scratch per point: ncol, m, m
+  unsigned long long *ns;
+};
+
+// src/ldpred2.cpp:9-69 (SAMPLING false) and src/ldpred2-sampling.cpp:9-59 (SAMPLING true) for point g = blockIdx.x, with
+// auto's warp-0 scan: lane l draws the uniform popc(lanes below l that draw) ahead of the state, a sparse point's lanes
+// with postp < p draw none, and the scan stops at the first lane that draws a normal or changes beta.
+template <bool SAMPLING>
+__global__ void __launch_bounds__(LT) k_ldpred2_grid(const long long *__restrict__ p, const int *__restrict__ rows,
+                                                     const int *__restrict__ first_i, const double *__restrict__ x, int ncol,
+                                                     const LdgArgs A) {
+  __shared__ lda_mat s_pw[32];  // A^(2^i)
+  __shared__ lda_mat s_ln[32];  // A^(o + 1): the draw o uniforms ahead is row 2 of it applied to the state
+  __shared__ int s_cmd;
+  __shared__ double s_shift;
+  const int g = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const unsigned long long t0 = globaltimer();
+  const int m = A.m, T = A.burn_in + A.num_iter;
+  double *dp = A.dot + (size_t)g * ncol, *cb = A.cb + (size_t)g * m, *avg = A.avg + (size_t)g * m;
+  if (tid == 0) lda_pow2_table(s_pw, 32);
+  for (int i = tid; i < ncol; i += LT) dp[i] = 0;
+  for (int i = tid; i < m; i += LT) cb[i] = 0, avg[i] = 0;
+  if (SAMPLING)
+    for (size_t i = tid; i < (size_t)m * A.num_iter; i += LT) A.sample[i] = 0;
+  __syncthreads();
+  if (tid < 32) s_ln[tid] = lda_mat_pow(s_pw, tid + 1);
+  __syncthreads();
+  // src/ldpred2.cpp:27-28
+  const double pp = A.p[g], h2_per_var = __ddiv_rn(A.h2[g], __dmul_rn((double)m, pp));
+  const double inv_odd_p = __ddiv_rn(__dsub_rn(1.0, pp), pp);
+  const int sparse = A.sparse[g] != 0;
+  // warp 0's chain state (every lane holds the same values)
+  uint32_t st[6];
+  for (int i = 0; i < 6; i++) st[i] = A.rng[6 * g + i];
+  double gap = 0;
+  bool diverged = false;
+  for (int k = 0; k < T; k++) {
+    gap = 0;
+    int j = 0;
+    for (;;) {
+      if (warp == 0) {
+        int cmd = CMD_NEXT_SWEEP;
+        double shift = 0;
+        while (j < m) {
+          const int jj = j + lane, nv = min(32, m - j);
+          const bool valid = jj < m;
+          lda_gcoord_t co = {0, 0, 0};
+          double cur = 0;
+          int j2 = 0;
+          if (valid) {
+            j2 = A.ind_sub[jj];
+            cur = cb[jj];
+            co = lda_grid_coord(lda_grid_res(A.beta_hat[jj], dp[j2], cur, SAMPLING), h2_per_var, A.n_vec[jj], inv_odd_p);
+          }
+          const bool draws = valid && lda_grid_draws(sparse, co.postp, pp);
+          const unsigned dmask = __ballot_sync(0xffffffffu, draws);
+          bool sel = false;
+          if (draws) {
+            const lda_mat *M = &s_ln[lda_grid_offset(dmask, lane)];
+            sel = co.postp > lda_u01(lda_mulmod3(M->a + 6, st, LDA_M1), lda_mulmod3(M->a + 15, st + 3, LDA_M2));
+          }
+          // the first lane that draws a normal or changes beta; the lanes before it only consume their uniforms
+          const unsigned stop = __ballot_sync(0xffffffffu, valid && (sel || cur != 0));
+          const int last = stop ? __ffs(stop) - 1 : nv - 1;
+          if (!SAMPLING && draws && lane <= last && k >= A.burn_in) avg[jj] = __dadd_rn(avg[jj], __dmul_rn(co.C3, co.postp));
+          const int used = __popc(dmask & (last == 31 ? 0xffffffffu : (2u << last) - 1));
+          if (used) lda_mat_apply(&s_ln[used - 1], st);
+          if (!stop) {
+            j += nv;
+            continue;
+          }
+          const bool lsel = __shfl_sync(0xffffffffu, sel, last);
+          const double lcur = __shfl_sync(0xffffffffu, cur, last), C3 = __shfl_sync(0xffffffffu, co.C3, last);
+          const double C4 = __shfl_sync(0xffffffffu, co.C4, last);
+          const int lj2 = __shfl_sync(0xffffffffu, j2, last);
+          double diff = -lcur, nbeta = 0;
+          if (lsel) {  // src/ldpred2.cpp:53-57, src/ldpred2-sampling.cpp:50-52
+            nbeta = lda_rnorm(C3, __dsqrt_rn(C4), st);
+            diff = __dadd_rn(diff, nbeta);
+            if (!SAMPLING) gap = __dadd_rn(gap, __dmul_rn(nbeta, nbeta));
+            if (SAMPLING && k >= A.burn_in && lane == 0) A.sample[(size_t)(k - A.burn_in) * m + j + last] = nbeta;
+          }
+          if (lane == 0) cb[j + last] = nbeta;
+          j += last + 1;
+          if (diff != 0) {
+            cmd = lj2;
+            shift = diff;
+            break;
+          }
+        }
+        if (!SAMPLING && cmd == CMD_NEXT_SWEEP && gap > A.gap0) cmd = CMD_DIVERGED;  // src/ldpred2.cpp:65
+        if (lane == 0) {
+          s_cmd = cmd;
+          s_shift = shift;
+        }
+      }
+      __syncthreads();
+      const int cmd = s_cmd;
+      if (cmd < 0) {
+        diverged = cmd == CMD_DIVERGED;
+        break;
+      }
+      incr_mult_col(p, rows, first_i, x, cmd, s_shift, dp, tid);
+      __syncthreads();
+    }
+    __syncthreads();  // s_cmd is rewritten by the next sweep
+    if (diverged) break;
+  }
+  if (!SAMPLING) {
+    const double inv = (double)A.num_iter;
+    for (int i = tid; i < m; i += LT) A.beta_est[(size_t)g * m + i] = diverged ? na_real() : __ddiv_rn(avg[i], inv);
+  }
+  if (tid == 0 && A.ns) A.ns[g] = globaltimer() - t0;
 }
 
 static int bind(const bsg_sfbm *s) {
   BSG_CUDA(cudaSetDevice(s->device));
+  return BSG_OK;
+}
+
+// MRG32k3a: each component below its modulus and not all zero
+static int check_rng(const unsigned *rng_state, int n, const char *what) {
+  for (int c = 0; c < n; c++) {
+    const unsigned *s = rng_state + 6 * c;
+    if (s[0] >= LDA_M1 || s[1] >= LDA_M1 || s[2] >= LDA_M1 || s[3] >= LDA_M2 || s[4] >= LDA_M2 || s[5] >= LDA_M2 ||
+        (s[0] | s[1] | s[2]) == 0 || (s[3] | s[4] | s[5]) == 0)
+      return fail(BSG_ERR_ARG, "rng_state of %s %d is not a valid MRG32k3a state.", what, c);
+  }
   return BSG_OK;
 }
 
@@ -874,6 +1008,17 @@ int bsg_ldpred2_auto(bsg_sfbm *corr, const double *beta_hat, const double *n_vec
                      const double *alpha_bounds, double mean_ld, const unsigned *rng_state, double *beta_est,
                      double *postp_est, double *corr_est, double *path_p, double *path_h2, double *path_alpha,
                      double *sample_beta, double *seconds) {
+  return bsg_ldpred2_auto_ex(corr, beta_hat, n_vec, log_var, m, ind_sub, nchain, p_init, h2_init, burn_in, num_iter,
+                             report_step, no_jump_sign, shrink_corr, use_mle, p_bounds, alpha_bounds, mean_ld, rng_state,
+                             beta_est, postp_est, corr_est, path_p, path_h2, path_alpha, sample_beta, seconds, nullptr);
+}
+
+int bsg_ldpred2_auto_ex(bsg_sfbm *corr, const double *beta_hat, const double *n_vec, const double *log_var, int m,
+                        const int *ind_sub, int nchain, const double *p_init, double h2_init, int burn_in, int num_iter,
+                        int report_step, int no_jump_sign, double shrink_corr, int use_mle, const double *p_bounds,
+                        const double *alpha_bounds, double mean_ld, const unsigned *rng_state, double *beta_est,
+                        double *postp_est, double *corr_est, double *path_p, double *path_h2, double *path_alpha,
+                        double *sample_beta, double *seconds, unsigned *rng_out) {
   if (!corr || m < 1 || nchain < 0) return fail(BSG_ERR_ARG, "null argument, m < 1 or nchain < 0");
   if (!beta_hat || !n_vec || !log_var || !ind_sub || !p_bounds || !alpha_bounds)
     return fail(BSG_ERR_ARG, "null argument");
@@ -887,12 +1032,7 @@ int bsg_ldpred2_auto(bsg_sfbm *corr, const double *beta_hat, const double *n_vec
   if (!(alpha_bounds[0] <= alpha_bounds[1]) || !std::isfinite(alpha_bounds[0]) || !std::isfinite(alpha_bounds[1]))
     return fail(BSG_ERR_ARG, "alpha_bounds must be finite with alpha_bounds[0] <= alpha_bounds[1].");
   if (!(mean_ld > 0)) return fail(BSG_ERR_ARG, "mean_ld must be positive.");
-  for (int c = 0; c < nchain; c++) {  // MRG32k3a: each component below its modulus and not all zero
-    const unsigned *s = rng_state + 6 * c;
-    if (s[0] >= LDA_M1 || s[1] >= LDA_M1 || s[2] >= LDA_M1 || s[3] >= LDA_M2 || s[4] >= LDA_M2 || s[5] >= LDA_M2 ||
-        (s[0] | s[1] | s[2]) == 0 || (s[3] | s[4] | s[5]) == 0)
-      return fail(BSG_ERR_ARG, "rng_state of chain %d is not a valid MRG32k3a state.", c);
-  }
+  BSG_TRY(check_rng(rng_state, nchain, "chain"));
   BSG_TRY(check_sub(corr, ind_sub, m));
   if (nchain == 0) return BSG_OK;
   BSG_TRY(bind(corr));
@@ -927,6 +1067,7 @@ int bsg_ldpred2_auto(bsg_sfbm *corr, const double *beta_hat, const double *n_vec
   if (e == cudaSuccess) e = b.alloc(&A.causal, mc);
   if (e == cudaSuccess && A.nrep) e = b.alloc(&A.sample, mc * A.nrep);
   if (e == cudaSuccess) e = b.alloc(&A.ns, (size_t)nchain);
+  if (e == cudaSuccess && rng_out) e = b.alloc(&A.rng_out, (size_t)6 * nchain);
   if (e != cudaSuccess) {
     cudaGetLastError();
     return fail(e == cudaErrorMemoryAllocation ? BSG_ERR_ALLOC : BSG_ERR_CUDA, "ldpred2_auto state (%s)", cudaGetErrorString(e));
@@ -942,11 +1083,81 @@ int bsg_ldpred2_auto(bsg_sfbm *corr, const double *beta_hat, const double *n_vec
   BSG_CUDA(cudaMemcpyAsync(path_h2, A.path_h2, tc * sizeof(double), cudaMemcpyDeviceToHost, st));
   BSG_CUDA(cudaMemcpyAsync(path_alpha, A.path_alpha, tc * sizeof(double), cudaMemcpyDeviceToHost, st));
   if (A.nrep) BSG_CUDA(cudaMemcpyAsync(sample_beta, A.sample, mc * A.nrep * sizeof(double), cudaMemcpyDeviceToHost, st));
+  if (rng_out) BSG_CUDA(cudaMemcpyAsync(rng_out, A.rng_out, (size_t)6 * nchain * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
   std::vector<unsigned long long> ns(nchain);
   BSG_CUDA(cudaMemcpyAsync(ns.data(), A.ns, (size_t)nchain * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
   BSG_CUDA(cudaStreamSynchronize(st));
   if (seconds)
     for (int c = 0; c < nchain; c++) seconds[c] = ns[c] * 1e-9;
+  return BSG_OK;
+}
+
+int bsg_ldpred2_grid(bsg_sfbm *corr, const double *beta_hat, const double *n_vec, int m, const int *ind_sub, int npoint,
+                     const double *p, const double *h2, const int *sparse, int burn_in, int num_iter, int sampling,
+                     const unsigned *rng_state, double *beta_est, double *sample_beta, double *seconds) {
+  if (!corr || m < 1 || npoint < 0) return fail(BSG_ERR_ARG, "null argument, m < 1 or npoint < 0");
+  if (!beta_hat || !n_vec || !ind_sub) return fail(BSG_ERR_ARG, "null argument");
+  if (npoint > 0 && (!p || !h2 || !sparse || !rng_state || (sampling ? !sample_beta : !beta_est)))
+    return fail(BSG_ERR_ARG, "null argument");
+  if (corr->nrow != corr->ncol) return fail(BSG_ERR_DIM, "Incompatibility between dimensions.");
+  if (burn_in < 0 || num_iter < 1 || (long long)burn_in + num_iter > INT_MAX)
+    return fail(BSG_ERR_ARG, "burn_in must be >= 0 and num_iter >= 1.");
+  if (sampling && npoint != 1)
+    return fail(BSG_ERR_ARG, "Only one set of parameters is allowed when using 'return_sampling_betas'.");
+  BSG_TRY(check_rng(rng_state, npoint, "point"));
+  BSG_TRY(check_sub(corr, ind_sub, m));
+  if (npoint == 0) return BSG_OK;
+  BSG_TRY(bind(corr));
+  double ss = 0;  // src/ldpred2.cpp:29-30, folded in order
+  for (int j = 0; j < m; j++) ss = ss + beta_hat[j] * beta_hat[j];
+  const size_t mp = (size_t)m * npoint, smp = sampling ? (size_t)m * num_iter : 0;
+  size_t fr = 0, tot = 0;
+  BSG_CUDA(cudaMemGetInfo(&fr, &tot));
+  const size_t need = ((size_t)corr->ncol * npoint + 3 * mp + smp + 2 * (size_t)m + 2 * (size_t)npoint) * sizeof(double) +
+                      (size_t)npoint * (sizeof(int) + 6 * sizeof(uint32_t) + sizeof(unsigned long long)) + (size_t)m * sizeof(int);
+  if (need > fr)
+    return fail(BSG_ERR_ALLOC, "ldpred2_grid needs %.0f bytes of device memory for %d points, %.0f are free.", (double)need,
+                npoint, (double)fr);
+  cudaStream_t st = corr->stream;
+  Bufs b;
+  LdgArgs A{};
+  A.m = m, A.burn_in = burn_in, A.num_iter = num_iter, A.gap0 = 2 * ss;
+  double *d_bh = nullptr, *d_n = nullptr, *d_p = nullptr, *d_h2 = nullptr;
+  int *d_sub = nullptr, *d_sp = nullptr;
+  uint32_t *d_rng = nullptr;
+  cudaError_t e = b.up(&d_bh, beta_hat, (size_t)m, st);
+  if (e == cudaSuccess) e = b.up(&d_n, n_vec, (size_t)m, st);
+  if (e == cudaSuccess) e = b.up(&d_sub, ind_sub, (size_t)m, st);
+  if (e == cudaSuccess) e = b.up(&d_p, p, (size_t)npoint, st);
+  if (e == cudaSuccess) e = b.up(&d_h2, h2, (size_t)npoint, st);
+  if (e == cudaSuccess) e = b.up(&d_sp, sparse, (size_t)npoint, st);
+  if (e == cudaSuccess) e = b.up(&d_rng, (const uint32_t *)rng_state, (size_t)6 * npoint, st);
+  if (e == cudaSuccess) e = b.alloc(&A.beta_est, mp);
+  if (e == cudaSuccess) e = b.alloc(&A.cb, mp);
+  if (e == cudaSuccess) e = b.alloc(&A.avg, mp);
+  if (e == cudaSuccess) e = b.alloc(&A.dot, (size_t)corr->ncol * npoint);
+  if (e == cudaSuccess && sampling) e = b.alloc(&A.sample, smp);
+  if (e == cudaSuccess) e = b.alloc(&A.ns, (size_t)npoint);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    return fail(e == cudaErrorMemoryAllocation ? BSG_ERR_ALLOC : BSG_ERR_CUDA, "ldpred2_grid state (%s)", cudaGetErrorString(e));
+  }
+  A.beta_hat = d_bh, A.n_vec = d_n, A.p = d_p, A.h2 = d_h2, A.sparse = d_sp, A.ind_sub = d_sub, A.rng = d_rng;
+  if (sampling)
+    k_ldpred2_grid<true><<<npoint, LT, 0, st>>>(corr->p, corr->rows, corr->first_i, corr->x, corr->ncol, A);
+  else
+    k_ldpred2_grid<false><<<npoint, LT, 0, st>>>(corr->p, corr->rows, corr->first_i, corr->x, corr->ncol, A);
+  count_launch();
+  BSG_CUDA(cudaGetLastError());
+  if (sampling)
+    BSG_CUDA(cudaMemcpyAsync(sample_beta, A.sample, smp * sizeof(double), cudaMemcpyDeviceToHost, st));
+  else
+    BSG_CUDA(cudaMemcpyAsync(beta_est, A.beta_est, mp * sizeof(double), cudaMemcpyDeviceToHost, st));
+  std::vector<unsigned long long> ns(npoint);
+  BSG_CUDA(cudaMemcpyAsync(ns.data(), A.ns, (size_t)npoint * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+  BSG_CUDA(cudaStreamSynchronize(st));
+  if (seconds)
+    for (int g = 0; g < npoint; g++) seconds[g] = ns[g] * 1e-9;
   return BSG_OK;
 }
 

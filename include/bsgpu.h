@@ -350,6 +350,31 @@ int bsg_ldpred2_auto(bsg_sfbm *corr, const double *beta_hat, const double *n_vec
                      const double *alpha_bounds, double mean_ld, const unsigned *rng_state, double *beta_est,
                      double *postp_est, double *corr_est, double *path_p, double *path_h2, double *path_alpha,
                      double *sample_beta, double *seconds);
+/* bsg_ldpred2_auto, and rng_out (NULL allowed) receives each chain's MRG32k3a state after its last sweep (6 words per
+ * chain, after the last sweep's rbeta and bootstrap, or after the diverging sweep): the state R/LDpred2.R:266-279 continues
+ * from in the same %dorng% iteration.  bsg_ldpred2_auto is this call with rng_out NULL. */
+int bsg_ldpred2_auto_ex(bsg_sfbm *corr, const double *beta_hat, const double *n_vec, const double *log_var, int m,
+                        const int *ind_sub, int nchain, const double *p_init, double h2_init, int burn_in, int num_iter,
+                        int report_step, int no_jump_sign, double shrink_corr, int use_mle, const double *p_bounds,
+                        const double *alpha_bounds, double mean_ld, const unsigned *rng_state, double *beta_est,
+                        double *postp_est, double *corr_est, double *path_p, double *path_h2, double *path_alpha,
+                        double *sample_beta, double *seconds, unsigned *rng_out);
+/* LDpred2-grid: src/ldpred2.cpp:9-69 (ldpred2_gibbs_one) for npoint grid points in one launch, one CTA per point, or with
+ * sampling, src/ldpred2-sampling.cpp:9-59 (ldpred2_gibbs_one_sampling) for one point.  beta_hat, n_vec: m values
+ * (R/LDpred2.R:89-91 passes beta / scale and n_eff); ind_sub: m 0-based columns of corr, any order, repeats allowed
+ * (BSG_ERR_BOUNDS out of range).  Point g runs with p[g], h2[g], sparse[g] (0 or not) and draws from the MRG32k3a state
+ * rng_state[6 g .. 6 g + 5]: one uniform per coordinate, none for a coordinate a sparse point zeroes (postp < p), and a
+ * normal by inversion when it is selected (DESIGN.md §4.18).  Every output of a point depends only on the inputs and its
+ * own state: bit-identical to the sequential CPU restatement.  Outputs: beta_est (m x npoint, column-major, without
+ * sampling): the average of C3 postp over the num_iter sweeps after burn_in, divided by num_iter, NA_real in the whole
+ * column when a sweep's sum of squared draws exceeds 2 sum(beta_hat^2); sample_beta (m x num_iter, with sampling): the
+ * coefficients after each sweep past burn_in; seconds[npoint] (NULL allowed): each point's device time.  m < 1,
+ * burn_in < 0, num_iter < 1, sampling with npoint != 1, an invalid state or a null pointer: BSG_ERR_ARG; a non-square
+ * corr: BSG_ERR_DIM; state larger than the free device memory (ncol + 3 m doubles per point, plus m x num_iter):
+ * BSG_ERR_ALLOC, with the bytes needed. */
+int bsg_ldpred2_grid(bsg_sfbm *corr, const double *beta_hat, const double *n_vec, int m, const int *ind_sub, int npoint,
+                     const double *p, const double *h2, const int *sparse, int burn_in, int num_iter, int sampling,
+                     const unsigned *rng_state, double *beta_est, double *sample_beta, double *seconds);
 
 /* ---- near-independent LD blocks (snp_ldsplit, R/split-LD.R:99-138) -------------------------------------------------- */
 /* Matrix::tril(corr) staged to HBM once: m x m lower triangle in CSC, p[m + 1] (non-decreasing, p[0] = 0), rows i
