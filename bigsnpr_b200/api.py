@@ -25,6 +25,7 @@ and error behaviour, so the parity tests read like the reference's testthat file
     snp_PRS / snp_grid_PRS   R/PRS.R:36-76, R/SCT.R:201-246 (bsg_prs_grid: every keep set of a chromosome in one call)
     big_univLinReg           bigstatsr's univLinReg5 + R glue (not vendored; bsg_univlinreg), result class MHTest
     big_univLogReg           bigstatsr's IRLS + R glue (not vendored; bsg_univlogreg, glm.fit null model and refits here)
+    big_spLinReg / big_spLogReg   bigstatsr's elastic net + CMSA (not vendored; bsg_splreg, DESIGN.md §4.19)
 
 Everything computes on the GPU through libbsgpu; there is no CPU path here (LD score regression, a few
 weighted least-squares fits on per-variant vectors, runs on the host).
@@ -2212,3 +2213,169 @@ def big_univLogReg(X, y01_train, ind_train=..., ind_col=..., covar_train=None, t
 def univlogreg_last_ms():
     """Device time of the last big_univLogReg call's IRLS (CUDA events), in ms."""
     return lib().bsg_univlogreg_last_ms()
+
+
+SPLREG_MESSAGES = ("Complete path", "No more improvement", "Too many variables")
+
+
+class SpModel:
+    """big_spLinReg's / big_spLogReg's result (bigstatsr's `big_sp_list`, power_scale = 1, power_adaptive = 0), one entry
+    per alpha, every coefficient on the original scale of the columns:
+
+    - `intercept[A]`, `beta[A][J]` (the kept columns `ind_col`, then the covariates): the mean over the K folds of each
+      fold's fit at its best lambda (cross-model selection and averaging);
+    - `validation_loss[A]`: the mean over folds of the best validation losses (mean squared error, or mean binomial
+      deviance); `nb_var[A]`: nonzero entries of `beta`;
+    - `message[A][K]`, `nb_lambda[A][K]` (lambda steps run), `best_lambda[A][K]` (0-based);
+    - `path[A][K]`: the whole path of each fit (`lambda`, `loss`, `nnz`, `passes`, and `beta` / `intercept` on the
+      standardised scale when the call asked for `return_path`);
+    - `center`, `scale`: the column statistics over ind.train of the kept columns then the covariates."""
+
+    def __init__(self, **kw):
+        self.__dict__.update(kw)
+
+    def summary(self, best_only=False):
+        """One row per alpha (dicts of alpha, intercept, beta, validation_loss, nb_var, message); best_only: the row of
+        the alpha with the lowest validation loss."""
+        rows = [dict(alpha=float(a), intercept=float(self.intercept[i]), beta=self.beta[i],
+                     validation_loss=float(self.validation_loss[i]), nb_var=int(self.nb_var[i]),
+                     message=list(self.message[i])) for i, a in enumerate(self.alphas)]
+        return rows[self.best_alpha] if best_only else rows
+
+    @property
+    def best_alpha(self):
+        return int(np.argmin(self.validation_loss))
+
+    def predict(self, X, ind_row=..., covar_row=None, base_row=None):
+        """The linear predictor of the best alpha's model at ind_row (also bigstatsr's default for logistic), plus the
+        offset base_row when given: the genotype part by bed_prodVec on the device, the covariates and the intercept on
+        the host.  A missing value on a (row, kept column) pair is refused, as in the fit."""
+        _assert_bed(X)
+        ind_row = X.rows_along() if ind_row is ... else _i32(ind_row)
+        i = self.best_alpha
+        G = self.ind_col.size
+        if G and not X.dosage_scale and bed_counts(X, ind_row, self.ind_col)[3].any():
+            raise ValueError("A kept column holds a missing value on 'ind.row'; impute it first (snp_fastImputeSimple).")
+        geno = bed_prodVec(X, self.beta[i][:G], ind_row, self.ind_col) if G else np.zeros(ind_row.size)
+        if np.isnan(geno).any():  # dosage tables: an NA code makes its output NaN
+            raise ValueError("A kept column holds a missing value on 'ind.row'; impute it first (snp_fastImputeSimple).")
+        out = geno + self.intercept[i]
+        if base_row is not None:
+            base = _f64(base_row).reshape(-1)
+            _assert_lengths(base, ind_row)
+            out = out + base
+        Kc = self.beta[i].size - G
+        if Kc:
+            if covar_row is None:
+                raise ValueError("'covar.row' is needed: the model has %d covariates." % Kc)
+            cv = _f64(covar_row).reshape(ind_row.size, Kc)
+            out = out + cv @ self.beta[i][G:]
+        return out
+
+
+def _big_spreg(family, X, y, ind_train, ind_col, covar_train, base_train, pf_X, pf_covar, alphas, K, ind_sets,
+               nlambda, lambda_min_ratio, nlam_min, n_abort, dfmax, eps, max_iter, power_scale, power_adaptive, seed,
+               return_path):
+    _assert_bed(X)
+    ind_train = X.rows_along() if ind_train is ... else _i32(ind_train)
+    ind_col = X.cols_along() if ind_col is ... else _i32(ind_col)
+    y = _f64(y).reshape(-1)
+    _assert_lengths(y, ind_train)
+    nr, nc = ind_train.size, ind_col.size
+    Kc = 0
+    cov = None
+    if covar_train is not None:
+        cv = np.asarray(covar_train, dtype=np.float64)
+        cv = cv.reshape(-1, 1) if cv.ndim == 1 else cv
+        if cv.shape[0] != nr:
+            raise ValueError(ERROR_DIM)
+        Kc = cv.shape[1]
+        cov = _f64(cv.T).reshape(-1)  # column-major
+    base = None if base_train is None else _f64(base_train).reshape(-1)
+    if base is not None:
+        _assert_lengths(base, ind_train)
+    pfx = None if pf_X is None else _f64(np.broadcast_to(np.asarray(pf_X, dtype=np.float64), (nc,)))
+    pfc = None if pf_covar is None else _f64(np.broadcast_to(np.asarray(pf_covar, dtype=np.float64), (Kc,)))
+    alphas = _f64(np.atleast_1d(alphas))
+    K = int(K)
+    if ind_sets is None:
+        ind_sets = (np.random.default_rng(seed).permutation(nr) % K + 1) if K >= 1 else np.ones(nr)
+    ind_sets = _i32(ind_sets)
+    _assert_lengths(ind_sets, ind_train)
+    A, F, Jmax = alphas.size, alphas.size * K, nc + Kc
+    center, scale, kept = np.empty(max(Jmax, 1)), np.empty(max(Jmax, 1)), np.zeros(max(nc, 1), dtype=np.uint8)
+    beta, b0 = np.zeros(max(F * Jmax, 1)), np.zeros(max(F, 1))
+    best, length, msg = (np.zeros(max(F, 1), dtype=np.int32) for _ in range(3))
+    lam, loss = np.zeros(max(F * nlambda, 1)), np.zeros(max(F * nlambda, 1))
+    nnz, npass = np.zeros(max(F * nlambda, 1), dtype=np.int32), np.zeros(max(F * nlambda, 1), dtype=np.int32)
+    pbeta = np.zeros(max(F * nlambda * Jmax, 1)) if return_path else None
+    pb0 = np.zeros(max(F * nlambda, 1)) if return_path else None
+    check(lib().bsg_splreg(X._h, _pi(ind_train), nr, _pi(ind_col), nc, family, _pd(y), _pd(cov), Kc, _pd(base),
+                           _pd(pfx), _pd(pfc), _pd(alphas), A, _pi(ind_sets), K, int(nlambda), float(lambda_min_ratio),
+                           int(nlam_min), int(n_abort), int(dfmax), float(eps), int(max_iter), float(power_scale),
+                           float(power_adaptive), _pd(center), _pd(scale), kept.ctypes.data_as(_lib.c_u8_p), _pd(beta),
+                           _pd(b0), _pi(best), _pi(length), _pi(msg), _pd(lam), _pd(loss), _pi(nnz), _pi(npass),
+                           _pd(pbeta), _pd(pb0)))
+    keep = kept[:nc].astype(bool)
+    J = int(keep.sum()) + Kc
+    cols = np.concatenate([np.flatnonzero(keep), nc + np.arange(Kc)])
+    c, s = center[cols], scale[cols]
+    beta = beta[:F * J].reshape(A, K, J)
+    raw = dict(beta=beta, b0=b0[:F].reshape(A, K), best=best[:F].reshape(A, K), length=length[:F].reshape(A, K),
+               message=msg[:F].reshape(A, K))
+    ob, oi = splreg_unscale(beta, raw["b0"], c, s)
+    path = [[None] * K for _ in range(A)]
+    for a in range(A):
+        for k in range(K):
+            f, L = a * K + k, int(length[a * K + k])
+            sl = slice(f * nlambda, f * nlambda + L)
+            p = dict(lambda_=lam[sl].copy(), loss=loss[sl].copy(), nnz=nnz[sl].copy(), passes=npass[sl].copy())
+            if return_path:
+                p["beta"] = pbeta[:F * nlambda * J].reshape(F, nlambda, J)[f, :L].copy()
+                p["intercept"] = pb0[sl].copy()
+            path[a][k] = p
+    best_loss = np.array([[path[a][k]["loss"][raw["best"][a, k]] for k in range(K)] for a in range(A)])
+    return SpModel(family="binomial" if family else "gaussian", alphas=alphas, intercept=oi, beta=ob,
+                   validation_loss=best_loss.mean(axis=1), nb_var=(ob != 0).sum(axis=1),
+                   message=[[SPLREG_MESSAGES[m] for m in raw["message"][a]] for a in range(A)],
+                   nb_lambda=raw["length"], best_lambda=raw["best"], path=path, ind_col=ind_col[keep],
+                   center=c, scale=s, ind_sets=ind_sets, raw=raw)
+
+
+def splreg_unscale(beta, b0, center, scale):
+    """Cross-model averaging on the original scale: per fit beta_j / s_j and b0 - sum_j c_j beta_j / s_j, then the mean
+    over folds.  beta [A][K][J] and b0 [A][K] on the standardised scale."""
+    bo = beta / scale
+    io = b0 - (bo * center).sum(axis=2)
+    return bo.mean(axis=1), io.mean(axis=1)
+
+
+def big_spLinReg(X, y_train, ind_train=..., ind_col=..., covar_train=None, base_train=None, pf_X=None, pf_covar=None,
+                 alphas=1, K=10, ind_sets=None, nlambda=200, lambda_min_ratio=1e-4, nlam_min=50, n_abort=10,
+                 dfmax=50000, eps=1e-5, max_iter=1000, power_scale=1, power_adaptive=0, seed=1, return_path=False,
+                 ncores=1):
+    """bigstatsr's big_spLinReg on the device (bsg_splreg): the elastic net (1/2n)|y - b0 - X beta|^2 +
+    lambda sum_j pf_j (alpha |beta_j| + (1 - alpha) / 2 beta_j^2) on standardised columns, K folds x alphas paths with
+    early stopping on each fold's held-out loss, averaged over folds (CMSA).  ind_sets fixes the folds; otherwise they
+    come from a permutation seeded by `seed` (R's sample is not reproduced).  Returns an SpModel."""
+    return _big_spreg(0, X, y_train, ind_train, ind_col, covar_train, base_train, pf_X, pf_covar, alphas, K, ind_sets,
+                      nlambda, lambda_min_ratio, nlam_min, n_abort, dfmax, eps, max_iter, power_scale, power_adaptive,
+                      seed, return_path)
+
+
+def big_spLogReg(X, y01_train, ind_train=..., ind_col=..., covar_train=None, base_train=None, pf_X=None, pf_covar=None,
+                 alphas=1, K=10, ind_sets=None, nlambda=200, lambda_min_ratio=1e-4, nlam_min=50, n_abort=10,
+                 dfmax=50000, eps=1e-5, max_iter=1000, power_scale=1, power_adaptive=0, seed=1, return_path=False,
+                 ncores=1):
+    """bigstatsr's big_spLogReg on the device (bsg_splreg): big_spLinReg's penalty with the mean negative binomial
+    log-likelihood as the loss, fitted by coordinate descent on a quadratic approximation whose weights p (1 - p) are
+    recomputed at the start of every pass.  y01_train must be 0 / 1.  Returns an SpModel; predict gives the linear
+    predictor."""
+    return _big_spreg(1, X, y01_train, ind_train, ind_col, covar_train, base_train, pf_X, pf_covar, alphas, K, ind_sets,
+                      nlambda, lambda_min_ratio, nlam_min, n_abort, dfmax, eps, max_iter, power_scale, power_adaptive,
+                      seed, return_path)
+
+
+def splreg_last_ms():
+    """Device time of the last big_spLinReg / big_spLogReg call (CUDA events), in ms."""
+    return lib().bsg_splreg_last_ms()

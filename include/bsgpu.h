@@ -291,6 +291,41 @@ int bsg_univlogreg(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, i
 /* device time in ms (CUDA events) of the last bsg_univlogreg: column checks to the last IRLS step, copies excluded */
 double bsg_univlogreg_last_ms(void);
 
+/* big_spLinReg (family 0) / big_spLogReg (family 1) with power_scale = 1, power_adaptive = 0 (bigstatsr's penalised
+ * regression, not vendored in the reference; DESIGN.md section 4.19, restated in tests/splreg_ref.py).  Every fit
+ * f = ia * K + k (alpha alphas[ia], fold k) runs on one 8-CTA thread-block cluster over the whole lambda path, state
+ * kept on the device; nr <= 1,048,576.
+ *   - Observations: ind_row (1-based, repeats allowed, NULL = all) with y[nr] (family 1: 0 / 1), covar nr x Kc
+ *     column-major, base[nr] offset (NULL = 0), ind_sets[nr] fold of each observation in 1..K (K >= 2; every fold leaves
+ *     at least two training observations and holds at least one).
+ *   - Columns: ind_col (1-based, NULL = all) then the Kc covariates.  center / scale [nc + Kc] are the mean and sd (divisor
+ *     nr) over all observations; genotype columns with scale <= 1e-8 are dropped (kept[nc] 0), the fit's J columns are the
+ *     kept ones in ind_col order, then the covariates (a constant covariate: BSG_ERR_ARG).  Fits use x~ = (x - c) / s.
+ *   - Penalty factors pf_X[nc], pf_covar[Kc] (NULL = 1); alphas in (0, 1].
+ *   - Per fit: the null fit of the intercept and pf = 0 columns, lambda_max = max |z_j| / (alpha pf_j) over pf_j > 0,
+ *     then nlambda values lambda_max * step^k, step = lambda_min_ratio^(1 / (nlambda - 1)), each from the previous
+ *     solution: sequential strong rule, coordinate-descent passes over the working set until
+ *     max |delta| <= eps * max |coef| (intercept included) or max_iter passes, a full KKT pass, repeat while a column
+ *     violates.  Stops at the first of: more than dfmax nonzero coefficients (message 2), the best validation loss
+ *     n_abort steps behind with at least nlam_min steps run (message 1), the end of the path (message 0).
+ * Outputs, J = (kept genotype columns) + Kc: beta [F][J] and intercept [F] at each fit's best lambda (standardised
+ * scale), best / length / message [F], lambda / loss (validation MSE or mean binomial deviance) / nnz / npass
+ * [F][nlambda] (entries past length are 0), path_beta [F][nlambda][J] and path_b0 [F][nlambda] when not NULL.
+ * Every sum over observations has one fixed order (8,192-position segments of 256-slot sums, added in order), so each
+ * fit's bytes depend on its problem alone.
+ * Refusals: power_scale != 1, power_adaptive != 0, alpha outside (0, 1], y01 not 0 / 1, non-finite y / covar / base,
+ * negative or non-finite penalty factors, invalid path parameters: BSG_ERR_ARG; indices out of range: BSG_ERR_BOUNDS;
+ * other FBM.code256 tables than hard calls and dosages: BSG_ERR_TYPE; scratch beyond free memory: BSG_ERR_ALLOC; all
+ * before any allocation.  An NA code on a selected (row, column) pair: BSG_ERR_ARG after the column-statistics pass. */
+int bsg_splreg(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, int nc, int family, const double *y,
+               const double *covar, int Kc, const double *base, const double *pf_X, const double *pf_covar,
+               const double *alphas, int nalpha, const int *ind_sets, int K, int nlambda, double lambda_min_ratio,
+               int nlam_min, int n_abort, int dfmax, double eps, int max_iter, double power_scale, double power_adaptive,
+               double *center, double *scale, uint8_t *kept, double *beta, double *intercept, int *best, int *length,
+               int *message, double *lambda, double *loss, int *nnz, int *npass, double *path_beta, double *path_b0);
+/* device time in ms (CUDA events) of the last bsg_splreg: column statistics to the end of the last fit */
+double bsg_splreg_last_ms(void);
+
 /* ---- sparse LD matrix (bigsparser's SFBM) and summary-statistics PRS -------------------------------------- */
 /* as_SFBM(corr[, compact]) staged to HBM once, in bigsparser's storage as bigsnpr reads it (src/ld-scores-sfbm.cpp:14-66):
  *   - p: ncol + 1 doubles, non-decreasing integers starting at 0 (X$p);
