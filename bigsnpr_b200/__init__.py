@@ -13,6 +13,7 @@ from .api import (  # noqa: F401
     snp_ld_scores, snp_scaleBinom, code256_dosage_scale, prod_and_rowSumsSq2,
     snp_projectSelfPCA, SFBM, as_SFBM, ld_scores_sfbm, seq_log, snp_lassosum2,
     LDCorr, snp_ldsplit, sp_solve_sym, snp_ldpred2_inf, snp_ldpred2_auto, snp_ldpred2_grid, snp_ldsc, snp_ldsc2, GridPRS, snp_PRS, snp_grid_PRS,
-    MHTest, big_univLinReg, big_univLogReg, SpModel, big_spLinReg, big_spLogReg)
+    MHTest, big_univLinReg, big_univLogReg, SpModel, big_spLinReg, big_spLogReg,
+    snp_grid_stacking)
 
 __all__ = [n for n in dir() if not n.startswith("_")]

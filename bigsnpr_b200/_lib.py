@@ -73,7 +73,13 @@ SIGNATURES = {
                              c_dbl_p, c_dbl_p, C.c_int, c_int_p, C.c_int, C.c_int, C.c_double, C.c_int, C.c_int, C.c_int,
                              C.c_double, C.c_int, C.c_double, C.c_double, c_dbl_p, c_dbl_p, c_u8_p, c_dbl_p, c_dbl_p,
                              c_int_p, c_int_p, c_int_p, c_dbl_p, c_dbl_p, c_int_p, c_int_p, c_dbl_p, c_dbl_p]),
+    "bsg_splreg_dense": (C.c_int, [vp, C.c_int, C.c_int64, C.c_int, C.c_int, c_int_p, C.c_int, c_int_p, C.c_int, C.c_int,
+                                   C.c_int, c_dbl_p, c_dbl_p, C.c_int, c_dbl_p, c_dbl_p, c_dbl_p, c_dbl_p, C.c_int, c_int_p,
+                                   C.c_int, C.c_int, C.c_double, C.c_int, C.c_int, C.c_int, C.c_double, C.c_int,
+                                   C.c_double, C.c_double, c_dbl_p, c_dbl_p, c_u8_p, c_dbl_p, c_dbl_p, c_int_p, c_int_p,
+                                   c_int_p, c_dbl_p, c_dbl_p, c_int_p, c_int_p, c_dbl_p, c_dbl_p]),
     "bsg_splreg_last_ms": (C.c_double, []),
+    "bsg_splreg_last_stage_ms": (C.c_double, []),
     "bsg_sfbm_open": (C.c_int, [C.c_int, C.c_int, c_dbl_p, c_dbl_p, c_int_p, C.c_int, C.POINTER(vp)]),
     "bsg_sfbm_close": (None, [vp]),
     "bsg_sfbm_nrow": (C.c_int, [vp]),

@@ -25,7 +25,8 @@ and error behaviour, so the parity tests read like the reference's testthat file
     snp_PRS / snp_grid_PRS   R/PRS.R:36-76, R/SCT.R:201-246 (bsg_prs_grid: every keep set of a chromosome in one call)
     big_univLinReg           bigstatsr's univLinReg5 + R glue (not vendored; bsg_univlinreg), result class MHTest
     big_univLogReg           bigstatsr's IRLS + R glue (not vendored; bsg_univlogreg, glm.fit null model and refits here)
-    big_spLinReg / big_spLogReg   bigstatsr's elastic net + CMSA (not vendored; bsg_splreg, DESIGN.md §4.19)
+    big_spLinReg / big_spLogReg   bigstatsr's elastic net + CMSA (not vendored; bsg_splreg / bsg_splreg_dense, DESIGN.md §4.19)
+    snp_grid_stacking        R/SCT.R:266-304 (big_spLinReg / big_spLogReg over snp_grid_PRS's scores, then the fold)
 
 Everything computes on the GPU through libbsgpu; there is no CPU path here (LD score regression, a few
 weighted least-squares fits on per-variant vectors, runs on the host).
@@ -2248,15 +2249,30 @@ class SpModel:
 
     def predict(self, X, ind_row=..., covar_row=None, base_row=None):
         """The linear predictor of the best alpha's model at ind_row (also bigstatsr's default for logistic), plus the
-        offset base_row when given: the genotype part by bed_prodVec on the device, the covariates and the intercept on
-        the host.  A missing value on a (row, kept column) pair is refused, as in the fit."""
-        _assert_bed(X)
-        ind_row = X.rows_along() if ind_row is ... else _i32(ind_row)
+        offset base_row when given.  On a Bed the genotype part is bed_prodVec on the device; on a dense float32 /
+        float64 matrix (what the model was fitted on) it is X[ind_row, ind_col] @ beta in float64 on the host, one pass
+        over the kept columns.  The covariates and the intercept are added on the host.  A missing value on a (row, kept
+        column) pair is refused, as in the fit."""
         i = self.best_alpha
         G = self.ind_col.size
-        if G and not X.dosage_scale and bed_counts(X, ind_row, self.ind_col)[3].any():
-            raise ValueError("A kept column holds a missing value on 'ind.row'; impute it first (snp_fastImputeSimple).")
-        geno = bed_prodVec(X, self.beta[i][:G], ind_row, self.ind_col) if G else np.zeros(ind_row.size)
+        if isinstance(X, Bed):
+            ind_row = X.rows_along() if ind_row is ... else _i32(ind_row)
+            if G and not X.dosage_scale and bed_counts(X, ind_row, self.ind_col)[3].any():
+                raise ValueError("A kept column holds a missing value on 'ind.row'; impute it first "
+                                 "(snp_fastImputeSimple).")
+            geno = bed_prodVec(X, self.beta[i][:G], ind_row, self.ind_col) if G else np.zeros(ind_row.size)
+        else:
+            X = _dense_matrix(X)
+            ind_row = np.arange(1, X.shape[0] + 1, dtype=np.int32) if ind_row is ... else _i32(ind_row)
+            for ind, lim in ((ind_row, X.shape[0]), (self.ind_col, X.shape[1])):
+                if ind.size and (ind.min() < 1 or ind.max() > lim):
+                    raise IndexError("subscript out of bounds")
+            geno = np.zeros(ind_row.size)
+            for c0 in range(0, G, 256):  # blocks of kept columns, so that no n x G copy is made
+                cols = self.ind_col[c0:c0 + 256] - 1
+                geno += X[np.ix_(ind_row - 1, cols)].astype(np.float64) @ self.beta[i][c0:c0 + cols.size]
+            if not np.isfinite(geno).all():
+                raise ValueError("A kept column holds a non-finite value on 'ind.row'.")
         if np.isnan(geno).any():  # dosage tables: an NA code makes its output NaN
             raise ValueError("A kept column holds a missing value on 'ind.row'; impute it first (snp_fastImputeSimple).")
         out = geno + self.intercept[i]
@@ -2273,12 +2289,39 @@ class SpModel:
         return out
 
 
+def _dense_matrix(X):
+    """X as a 2-D float32 / float64 array (an np.memmap or a GridPRS stays what it is); other types: TypeError."""
+    X = X if isinstance(X, np.ndarray) else np.asarray(X)
+    if X.dtype not in (np.float32, np.float64):
+        raise TypeError("A dense matrix must hold float32 or float64 values (not %s)." % X.dtype)
+    if X.ndim != 2:
+        raise ValueError(ERROR_DIM)
+    return X
+
+
+def _dense_operand(X):
+    """(X, dtype code, leading dimension) for bsg_splreg_dense: a column-major matrix (columns may sit ld >= nrow
+    elements apart, as in a column slice of a larger one) is passed as it is; any other layout, a C-ordered array
+    included, is first copied into a Fortran-ordered one."""
+    X = _dense_matrix(X)
+    n, it = X.shape[0], X.itemsize
+    st0, st1 = X.strides
+    if not (X.size == 0 or ((st0 == it or n == 1) and st1 % it == 0 and st1 >= max(n, 1) * it)):
+        X = np.asfortranarray(X)
+        st1 = max(n, 1) * it
+    return X, int(X.dtype == np.float64), (st1 // it if X.size else max(n, 1))
+
+
 def _big_spreg(family, X, y, ind_train, ind_col, covar_train, base_train, pf_X, pf_covar, alphas, K, ind_sets,
                nlambda, lambda_min_ratio, nlam_min, n_abort, dfmax, eps, max_iter, power_scale, power_adaptive, seed,
                return_path):
-    _assert_bed(X)
-    ind_train = X.rows_along() if ind_train is ... else _i32(ind_train)
-    ind_col = X.cols_along() if ind_col is ... else _i32(ind_col)
+    if isinstance(X, Bed):
+        nrow, ncol = X.nrow, X.ncol
+    else:
+        X, dtype, ld = _dense_operand(X)
+        nrow, ncol = X.shape
+    ind_train = np.arange(1, nrow + 1, dtype=np.int32) if ind_train is ... else _i32(ind_train)
+    ind_col = np.arange(1, ncol + 1, dtype=np.int32) if ind_col is ... else _i32(ind_col)
     y = _f64(y).reshape(-1)
     _assert_lengths(y, ind_train)
     nr, nc = ind_train.size, ind_col.size
@@ -2310,12 +2353,16 @@ def _big_spreg(family, X, y, ind_train, ind_col, covar_train, base_train, pf_X, 
     nnz, npass = np.zeros(max(F * nlambda, 1), dtype=np.int32), np.zeros(max(F * nlambda, 1), dtype=np.int32)
     pbeta = np.zeros(max(F * nlambda * Jmax, 1)) if return_path else None
     pb0 = np.zeros(max(F * nlambda, 1)) if return_path else None
-    check(lib().bsg_splreg(X._h, _pi(ind_train), nr, _pi(ind_col), nc, family, _pd(y), _pd(cov), Kc, _pd(base),
-                           _pd(pfx), _pd(pfc), _pd(alphas), A, _pi(ind_sets), K, int(nlambda), float(lambda_min_ratio),
-                           int(nlam_min), int(n_abort), int(dfmax), float(eps), int(max_iter), float(power_scale),
-                           float(power_adaptive), _pd(center), _pd(scale), kept.ctypes.data_as(_lib.c_u8_p), _pd(beta),
-                           _pd(b0), _pi(best), _pi(length), _pi(msg), _pd(lam), _pd(loss), _pi(nnz), _pi(npass),
-                           _pd(pbeta), _pd(pb0)))
+    tail = (family, _pd(y), _pd(cov), Kc, _pd(base), _pd(pfx), _pd(pfc), _pd(alphas), A, _pi(ind_sets), K, int(nlambda),
+            float(lambda_min_ratio), int(nlam_min), int(n_abort), int(dfmax), float(eps), int(max_iter),
+            float(power_scale), float(power_adaptive), _pd(center), _pd(scale), kept.ctypes.data_as(_lib.c_u8_p),
+            _pd(beta), _pd(b0), _pi(best), _pi(length), _pi(msg), _pd(lam), _pd(loss), _pi(nnz), _pi(npass), _pd(pbeta),
+            _pd(pb0))
+    if isinstance(X, Bed):
+        check(lib().bsg_splreg(X._h, _pi(ind_train), nr, _pi(ind_col), nc, *tail))
+    else:
+        check(lib().bsg_splreg_dense(C.c_void_p(X.ctypes.data) if X.size else None, dtype, ld, nrow, ncol,
+                                     _pi(ind_train), nr, _pi(ind_col), nc, 0, *tail))
     keep = kept[:nc].astype(bool)
     J = int(keep.sum()) + Kc
     cols = np.concatenate([np.flatnonzero(keep), nc + np.arange(Kc)])
@@ -2357,7 +2404,12 @@ def big_spLinReg(X, y_train, ind_train=..., ind_col=..., covar_train=None, base_
     """bigstatsr's big_spLinReg on the device (bsg_splreg): the elastic net (1/2n)|y - b0 - X beta|^2 +
     lambda sum_j pf_j (alpha |beta_j| + (1 - alpha) / 2 beta_j^2) on standardised columns, K folds x alphas paths with
     early stopping on each fold's held-out loss, averaged over folds (CMSA).  ind_sets fixes the folds; otherwise they
-    come from a permutation seeded by `seed` (R's sample is not reproduced).  Returns an SpModel."""
+    come from a permutation seeded by `seed` (R's sample is not reproduced).  Returns an SpModel.
+
+    X is a Bed, or a 2-D float32 / float64 matrix (an ndarray, np.memmap or GridPRS; bsg_splreg_dense): X[ind_train,
+    ind_col] is read once into device memory in its own type and widened to double exactly when read, so the fit is
+    the one of X.astype(float64).  A Fortran-ordered matrix is read in place; a C-ordered one is copied into Fortran
+    order first.  Non-finite values on the selected cells are refused."""
     return _big_spreg(0, X, y_train, ind_train, ind_col, covar_train, base_train, pf_X, pf_covar, alphas, K, ind_sets,
                       nlambda, lambda_min_ratio, nlam_min, n_abort, dfmax, eps, max_iter, power_scale, power_adaptive,
                       seed, return_path)
@@ -2379,3 +2431,55 @@ def big_spLogReg(X, y01_train, ind_train=..., ind_col=..., covar_train=None, bas
 def splreg_last_ms():
     """Device time of the last big_spLinReg / big_spLogReg call (CUDA events), in ms."""
     return lib().bsg_splreg_last_ms()
+
+
+def splreg_last_stage_ms():
+    """Host time of the last big_spLinReg / big_spLogReg call's staging (a dense matrix's gather and upload), in ms."""
+    return lib().bsg_splreg_last_stage_ms()
+
+
+def stacking_fold(w, lpS, grid_lpS_thr, betas, all_keep):
+    """R/SCT.R:283-296: per-SNP effects from the stacking weights w (one per column of snp_grid_PRS's matrix).  Keep set
+    s (chromosome-major, the order of unlist(all_keep)) owns columns s n_thr .. (s + 1) n_thr - 1; each of its SNPs gets
+    c(0, cumsum(b))[1 + sum(lp > grid_lpS_thr)] of that set's weights b (cumsum in long double, as R's), added over the
+    sets that hold it; beta.G = coef * betas.  A NaN lpS inside a set gives a NaN coefficient (R's NA index); SNPs in
+    no set get 0 * beta (NaN for a NaN beta)."""
+    thr = np.asarray(grid_lpS_thr, dtype=np.float64).reshape(-1)
+    lpS, betas, w = (np.asarray(v, dtype=np.float64).reshape(-1) for v in (lpS, betas, w))
+    nthr = thr.size
+    coef = np.zeros(betas.size)
+    s = 0
+    for chrom in all_keep:
+        for keep in chrom:
+            keep = np.asarray(keep, dtype=np.int64).reshape(-1) - 1
+            b2 = np.concatenate([[0.0], np.cumsum(w[s:s + nthr].astype(np.longdouble)).astype(np.float64)])
+            lp = lpS[keep]
+            add = b2[(lp[:, None] > thr).sum(axis=1)]
+            add[np.isnan(lp)] = np.nan
+            coef[keep] = coef[keep] + add
+            s += nthr
+    if s != w.size:
+        raise ValueError("'multi_PRS' has %d columns; its keep sets and thresholds make %d." % (w.size, s))
+    return coef * betas
+
+
+def snp_grid_stacking(multi_PRS, y_train, alphas=(1, 0.01, 0.0001), ncores=1, **kw):
+    """R/SCT.R:266-304: stacking over snp_grid_PRS's C+T scores.  big_spLogReg when y_train has exactly two distinct
+    values (they must be 0 / 1), big_spLinReg otherwise, over the dense score matrix on the device (**kw forwarded:
+    K, covar_train, pf_covar, ind_train, ind_col, ind_sets, seed, ...); then the best alpha's weights of the kept
+    columns are folded into per-SNP effects (stacking_fold).  Returns R's list: `intercept`, `beta.G`, `beta.covar`,
+    `mod` (the SpModel)."""
+    attrs = [getattr(multi_PRS, a, None) for a in ("lpS", "grid_lpS_thr", "betas", "all_keep")]
+    if any(a is None for a in attrs):
+        raise ValueError("'multi_PRS' must be the result of snp_grid_PRS (attributes lpS, grid_lpS_thr, betas, "
+                         "all_keep).")
+    lpS, thr, betas, all_keep = attrs
+    y = _f64(y_train).reshape(-1)
+    fit = big_spLogReg if np.unique(y).size == 2 else big_spLinReg
+    mod = fit(multi_PRS, y, alphas=alphas, ncores=ncores, **kw)
+    best = mod.summary(best_only=True)
+    G = mod.ind_col.size
+    w = np.zeros(multi_PRS.shape[1])
+    w[mod.ind_col - 1] = best["beta"][:G]
+    return {"intercept": best["intercept"], "beta.G": stacking_fold(w, lpS, thr, betas, all_keep),
+            "beta.covar": best["beta"][G:], "mod": mod}

@@ -16,6 +16,7 @@
 // column order.  Every floating operation is an __d*_rn intrinsic (no contraction) and exp / log are the shared fdlibm
 // restatement, so the NumPy and C restatements in tests/ reproduce the device byte for byte.
 #include <algorithm>
+#include <chrono>
 #include <cmath>
 #include <math.h>
 #include <vector>
@@ -38,6 +39,8 @@ constexpr int CS = 8;      // CTAs per fit (one thread-block cluster)
 constexpr int SL = 16;     // segments one CTA may own: n_train <= SEG * CS * SL
 constexpr int64_t NMAX = (int64_t)SEG * CS * SL;
 
+// The column sources, a compile-time parameter of both kernels: columns j < G come from the source, columns j >= G are
+// the covariates.  Cols reads the resident genotypes; Dense<T> reads a staged column-major block of float or double.
 struct Cols {
   const uint8_t *P;    // hard calls: copy A; dosages: the value copy
   int64_t stride;
@@ -48,12 +51,43 @@ struct Cols {
   int nr, G;
 };
 
+template <class T>
+struct Dense {
+  const T *X;          // [ncol][nr] the staged block: X[ind_row, ind_col], column-major by observation
+  const int *lines;    // [G] columns of the block
+  const double *cov;   // [J - G][nr] covariates, column-major by observation
+  int nr, G;
+};
+
 // column j at observation o, sample row `row`
 __device__ __forceinline__ double xraw(const Cols &c, int j, int o, int row) {
   if (j >= c.G) return c.cov[(int64_t)(j - c.G) * c.nr + o];
   const uint8_t *p = c.P + (int64_t)c.lines[j] * c.stride;
   if (c.D > 0) return __ddiv_rn((double)p[row], c.D);
   return (double)((p[row >> 2] >> (2 * (row & 3))) & 3);
+}
+
+// the block is staged by observation, so the sample row is not needed; float widens to double exactly
+template <class T>
+__device__ __forceinline__ double xraw(const Dense<T> &c, int j, int o, int) {
+  if (j >= c.G) return c.cov[(int64_t)(j - c.G) * c.nr + o];
+  return (double)c.X[(int64_t)c.lines[j] * c.nr + o];
+}
+
+__device__ __forceinline__ int row_of(const Cols &c, int o) { return c.rows[o]; }
+template <class T>
+__device__ __forceinline__ int row_of(const Dense<T> &, int o) { return o; }
+
+// a refused cell of column j < G at observation o: an NA code, or a non-finite value
+__device__ __forceinline__ bool cell_bad(const Cols &c, int j, int o, const uint8_t *raw, int n, const int *lut) {
+  const int row = c.rows[o];
+  if (c.D > 0) return lut[raw[(int64_t)c.lines[j] * n + row]] < 0;
+  return ((c.P[(int64_t)c.lines[j] * c.stride + (row >> 2)] >> (2 * (row & 3))) & 3) == 3;
+}
+
+template <class T>
+__device__ __forceinline__ bool cell_bad(const Dense<T> &c, int j, int o, const uint8_t *, int, const int *) {
+  return !isfinite(c.X[(int64_t)c.lines[j] * c.nr + o]);
 }
 
 // the 256-slot sum of f(b .. e-1) by one warp (slot t: positions b + t, b + t + 256, ...; then the halving tree)
@@ -89,22 +123,18 @@ __device__ __forceinline__ double warp_sum(int n, F f) {
   return tot;
 }
 
-__global__ void __launch_bounds__(ST) k_sp_stats(const Cols c, int J, const uint8_t *raw, int n, const int *lut,
+template <class Src>
+__global__ void __launch_bounds__(ST) k_sp_stats(const Src c, int J, const uint8_t *raw, int n, const int *lut,
                                                  double *center, double *scale, uint8_t *na) {
   const int j = blockIdx.x * (ST / 32) + (threadIdx.x >> 5);
   if (j >= J) return;
   int bad = 0;
-  if (j < c.G) {
-    for (int o = threadIdx.x & 31; o < c.nr; o += 32) {
-      const int row = c.rows[o];
-      if (c.D > 0) bad |= lut[raw[(int64_t)c.lines[j] * n + row]] < 0;
-      else bad |= ((c.P[(int64_t)c.lines[j] * c.stride + (row >> 2)] >> (2 * (row & 3))) & 3) == 3;
-    }
-  }
+  if (j < c.G)
+    for (int o = threadIdx.x & 31; o < c.nr; o += 32) bad |= cell_bad(c, j, o, raw, n, lut);
   bad = __any_sync(0xffffffffu, bad);
-  const double ctr = __ddiv_rn(warp_sum(c.nr, [&](int o) { return xraw(c, j, o, c.rows[o]); }), (double)c.nr);
+  const double ctr = __ddiv_rn(warp_sum(c.nr, [&](int o) { return xraw(c, j, o, row_of(c, o)); }), (double)c.nr);
   const double var = __ddiv_rn(warp_sum(c.nr, [&](int o) {
-    const double d = __dsub_rn(xraw(c, j, o, c.rows[o]), ctr);
+    const double d = __dsub_rn(xraw(c, j, o, row_of(c, o)), ctr);
     return __dmul_rn(d, d);
   }), (double)c.nr);
   if ((threadIdx.x & 31) == 0) {
@@ -114,8 +144,9 @@ __global__ void __launch_bounds__(ST) k_sp_stats(const Cols c, int J, const uint
   }
 }
 
+template <class Src>
 struct FArgs {
-  Cols c;
+  Src c;
   int J;
   const double *center, *iscale, *pf;  // [J]
   const double *y, *base;              // [nr] by observation
@@ -162,7 +193,8 @@ struct Smem {
 // sum; every CTA then adds all segment sums in segment order through distributed shared memory, so all CTAs hold the
 // same bits and take the same decisions.  Column loops over all positions (the full pass) give whole columns to warps,
 // columns split over the cluster.
-__global__ void __launch_bounds__(ST) k_splreg(const FArgs a) {
+template <class Src>
+__global__ void __launch_bounds__(ST) k_splreg(const FArgs<Src> a) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
   Smem &sm = *reinterpret_cast<Smem *>(smem_raw);
   cg::cluster_group cl = cg::this_cluster();
@@ -446,7 +478,7 @@ __global__ void __launch_bounds__(ST) k_splreg(const FArgs a) {
   }
 }
 
-static thread_local double g_last_ms = 0;
+static thread_local double g_last_ms = 0, g_stage_ms = 0;
 
 struct Events {
   cudaEvent_t ev[2] = {nullptr, nullptr};
@@ -462,28 +494,126 @@ static bool finite_all(const double *p, int64_t n) {
   return true;
 }
 
-}  // namespace splreg
-}  // namespace bsg
+static int scratch_fail(cudaError_t err) {
+  cudaGetLastError();
+  return fail(err == cudaErrorMemoryAllocation ? BSG_ERR_ALLOC : BSG_ERR_CUDA, "big_spLinReg scratch (%s)",
+              cudaGetErrorString(err));
+}
 
-using namespace bsg;
+// What an entry point hands the driver: the kernels' column source Src, the bounds n / m of ind_row / ind_col, the
+// stream, the device bytes stage() allocates (counted in the memory check), stage() itself (makes the nc selected columns
+// readable as source columns 0..nc-1 for the statistics), line() (the source column of selected column c in the fit),
+// what k_sp_stats' NA-code check reads, and the refusal of a flagged column.
 
-extern "C" {
+// the resident genotypes of a handle: hard calls, or the value copy of a dosage FBM
+struct BedOp {
+  using Src = Cols;
+  bsg_bed *h;
+  int n, m;
+  cudaStream_t s;
+  const uint8_t *raw;
+  const int *lut = nullptr;
+  const char *bad_msg = "Column %d holds a missing value on a training row; impute it first (snp_fastImputeSimple).";
+  size_t stage_bytes(int, int) const { return 0; }
+  int stage(const std::vector<int> &row0, const std::vector<int> &col0, int nc, Bufs &b, Cols &cs) {
+    const bool dos = h->fbm_generic != 0;
+    if (dos) BSG_TRY(dosage_build(h));
+    int *d_rows, *d_cols, *d_lut = nullptr;
+    cudaError_t err = b.up(&d_rows, row0, s);
+    if (err == cudaSuccess) err = b.up(&d_cols, col0.data(), (size_t)nc, s);
+    if (dos) {
+      std::vector<int> tab(256);
+      for (int c = 0; c < 256; c++)
+        tab[c] = h->code256[c] != h->code256[c] ? -1 : (int)nearbyint(h->dos_scale * h->code256[c]);
+      if (err == cudaSuccess) err = b.up(&d_lut, tab, s);
+    }
+    if (err != cudaSuccess) return scratch_fail(err);
+    lut = d_lut;
+    cs.P = dos ? h->dosV : h->A;
+    cs.stride = dos ? h->dosStride : h->strideA;
+    cs.D = dos ? (double)h->dos_scale : 0.0;
+    cs.rows = d_rows, cs.lines = d_cols;
+    return BSG_OK;
+  }
+  int line(int c, const std::vector<int> &col0) const { return col0[c]; }
+};
 
-int bsg_splreg(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, int nc, int family, const double *y,
-               const double *covar, int Kc, const double *base, const double *pf_X, const double *pf_covar,
-               const double *alphas, int nalpha, const int *ind_sets, int K, int nlambda, double lambda_min_ratio,
-               int nlam_min, int n_abort, int dfmax, double eps, int max_iter, double power_scale, double power_adaptive,
-               double *center, double *scale, uint8_t *kept, double *beta, double *intercept, int *best, int *length,
-               int *message, double *lambda, double *loss, int *nnz, int *npass, double *path_beta, double *path_b0) {
-  using namespace splreg;
-  if (!h) return fail(BSG_ERR_ARG, "null handle");
-  const bool dos = h->fbm_generic != 0;
-  if (dos && !h->dos_scale)
-    return fail(BSG_ERR_TYPE, "big_spLinReg / big_spLogReg on the device need hard calls or dosages (codes multiples of "
-                              "1 / D); this FBM.code256 holds other values.");
-  BSG_TRY(bind_device(h));
-  if (!ind_row) nr = h->n;
-  if (!ind_col) nc = h->m;
+// pinned host buffers of the dense staging, freed with their events
+struct Pinned {
+  void *p[2] = {nullptr, nullptr};
+  cudaEvent_t ev[2] = {nullptr, nullptr};
+  ~Pinned() {
+    for (int i = 0; i < 2; i++) {
+      if (ev[i]) cudaEventSynchronize(ev[i]), cudaEventDestroy(ev[i]);
+      if (p[i]) cudaFreeHost(p[i]);
+    }
+  }
+};
+
+// a host column-major matrix of T (leading dimension ld): X[ind_row, ind_col] is gathered into pinned chunks of whole
+// columns and uploaded once, so the block lives on the device as nc columns of nr observations
+template <class T>
+struct DenseOp {
+  using Src = Dense<T>;
+  static constexpr size_t CHUNK = (size_t)64 << 20;  // bytes per pinned buffer (two of them)
+  const T *X;
+  int64_t ld;
+  int n, m;
+  cudaStream_t s;
+  const uint8_t *raw = nullptr;
+  const int *lut = nullptr;
+  const char *bad_msg = "Column %d holds a non-finite value on a training row.";
+  size_t stage_bytes(int nr, int nc) const { return (size_t)nr * nc * sizeof(T) + (size_t)nc * sizeof(int); }
+  int stage(const std::vector<int> &row0, const std::vector<int> &col0, int nc, Bufs &b, Dense<T> &cs) {
+    const int nr = (int)row0.size();
+    std::vector<int> iota(nc);
+    for (int c = 0; c < nc; c++) iota[c] = c;
+    T *d_X;
+    int *d_cols;
+    cudaError_t err = b.alloc(&d_X, (size_t)nr * nc);
+    if (err == cudaSuccess) err = b.up(&d_cols, iota, s);
+    if (err != cudaSuccess) return scratch_fail(err);
+    bool contiguous = true;  // ind_row a run of consecutive rows: one copy per column
+    for (int r = 1; r < nr && contiguous; r++) contiguous = row0[r] == row0[0] + r;
+    const size_t colb = (size_t)nr * sizeof(T);
+    const int per = (int)std::max<size_t>(1, std::min<size_t>(CHUNK / std::max<size_t>(colb, 1), (size_t)nc));
+    Pinned pin;
+    for (int i = 0; i < 2 && nc > 0; i++) {
+      BSG_CUDA(cudaMallocHost(&pin.p[i], (size_t)per * colb));
+      BSG_CUDA(cudaEventCreateWithFlags(&pin.ev[i], cudaEventDisableTiming));
+    }
+    for (int c0 = 0, u = 0; c0 < nc; c0 += per, u ^= 1) {
+      const int cnt = std::min(per, nc - c0);
+      BSG_CUDA(cudaEventSynchronize(pin.ev[u]));
+      T *dst = static_cast<T *>(pin.p[u]);
+      for (int c = 0; c < cnt; c++, dst += nr) {
+        const T *src = X + (int64_t)col0[c0 + c] * ld;
+        if (contiguous) std::copy(src + row0[0], src + row0[0] + nr, dst);
+        else
+          for (int r = 0; r < nr; r++) dst[r] = src[row0[r]];
+      }
+      BSG_CUDA(cudaMemcpyAsync(d_X + (size_t)c0 * nr, pin.p[u], (size_t)cnt * colb, cudaMemcpyHostToDevice, s));
+      BSG_CUDA(cudaEventRecord(pin.ev[u], s));
+    }
+    BSG_CUDA(cudaStreamSynchronize(s));
+    cs.X = d_X, cs.lines = d_cols;
+    return BSG_OK;
+  }
+  int line(int c, const std::vector<int> &) const { return c; }
+};
+
+// validation, folds, memory check, staging, column statistics, the fits' launch, read-back and unpermute, for any
+// operand (bsg_splreg and bsg_splreg_dense)
+template <class Op>
+static int splreg_drive(Op &op, const int *ind_row, int nr, const int *ind_col, int nc, int family, const double *y,
+                        const double *covar, int Kc, const double *base, const double *pf_X, const double *pf_covar,
+                        const double *alphas, int nalpha, const int *ind_sets, int K, int nlambda,
+                        double lambda_min_ratio, int nlam_min, int n_abort, int dfmax, double eps, int max_iter,
+                        double power_scale, double power_adaptive, double *center, double *scale, uint8_t *kept,
+                        double *beta, double *intercept, int *best, int *length, int *message, double *lambda,
+                        double *loss, int *nnz, int *npass, double *path_beta, double *path_b0) {
+  if (!ind_row) nr = op.n;
+  if (!ind_col) nc = op.m;
   if (nr < 2 || nc < 0 || Kc < 0 || (Kc > 0 && !covar)) return fail(BSG_ERR_ARG, "Incompatibility between dimensions.");
   if (family != 0 && family != 1) return fail(BSG_ERR_ARG, "family must be 0 (linear) or 1 (logistic).");
   if (power_scale != 1.0) return fail(BSG_ERR_ARG, "Only 'power_scale = 1' is supported on the device.");
@@ -498,7 +628,7 @@ int bsg_splreg(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, int n
   if (!y || !ind_sets || !center || !scale || !kept || !beta || !intercept || !best || !length || !message || !lambda ||
       !loss || !nnz || !npass)
     return fail(BSG_ERR_ARG, "null argument");
-  const int n = h->n;
+  const int n = op.n;
   std::vector<int> row0(nr);
   for (int r = 0; r < nr; r++) {
     const int i = ind_row ? ind_row[r] : r + 1;
@@ -508,7 +638,7 @@ int bsg_splreg(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, int n
   std::vector<int> col0(std::max(nc, 1));
   for (int c = 0; c < nc; c++) {
     const int j = ind_col ? ind_col[c] : c + 1;
-    if (j < 1 || j > h->m) return fail(BSG_ERR_BOUNDS, "Tested subscript out of bounds (%d not in 1..%d).", j, h->m);
+    if (j < 1 || j > op.m) return fail(BSG_ERR_BOUNDS, "Tested subscript out of bounds (%d not in 1..%d).", j, op.m);
     col0[c] = j - 1;
   }
   if (!finite_all(y, nr)) return fail(BSG_ERR_ARG, "'y.train' must be finite.");
@@ -544,47 +674,35 @@ int bsg_splreg(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, int n
   const size_t need = (size_t)nr * (4 + 8 + 8 + 4 * K) + (size_t)Jall * (4 + 8 * 2 + 1) +
                       (size_t)F * ((size_t)nr * 8 * (family == 1 ? 3 : 1) + (size_t)Jall * (8 * 4 + (1 + 4) * CS) +
                                    (size_t)nlambda * 24 + 32) +
-                      (path_beta ? (size_t)F * nlambda * Jall * 8 : 0) + (1 << 20);
+                      (path_beta ? (size_t)F * nlambda * Jall * 8 : 0) + op.stage_bytes(nr, nc) + (1 << 20);
   size_t fr = 0, tot = 0;
   BSG_CUDA(cudaMemGetInfo(&fr, &tot));
   if (need > fr)
     return fail(BSG_ERR_ALLOC, "big_spLinReg / big_spLogReg need %.0f bytes of device memory (%d fits, %d observations, "
-                               "%d columns), %.0f are free.", (double)need, F, nr, Jall, (double)fr);
-  if (dos) BSG_TRY(dosage_build(h));
-  cudaStream_t s = h->stream;
+                               "%d columns, %.0f bytes staged), %.0f are free.", (double)need, F, nr, Jall,
+                (double)op.stage_bytes(nr, nc), (double)fr);
+  cudaStream_t s = op.s;
   std::vector<double> zero(nr, 0.0);
   Bufs b;
-  int *d_rows, *d_cols, *d_lut = nullptr;
+  typename Op::Src cs{};
+  const auto t0 = std::chrono::steady_clock::now();
+  BSG_TRY(op.stage(row0, col0, nc, b, cs));
+  g_stage_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
   double *d_cov = nullptr, *d_ctr, *d_sc;
   uint8_t *d_na;
-  cudaError_t err = b.up(&d_rows, row0, s);
-  if (err == cudaSuccess) err = b.up(&d_cols, col0.data(), (size_t)nc, s);
-  if (err == cudaSuccess && Kc > 0) err = b.up(&d_cov, covar, (size_t)nr * Kc, s);
+  cudaError_t err = cudaSuccess;
+  if (Kc > 0) err = b.up(&d_cov, covar, (size_t)nr * Kc, s);
   if (err == cudaSuccess) err = b.alloc(&d_ctr, (size_t)Jall);
   if (err == cudaSuccess) err = b.alloc(&d_sc, (size_t)Jall);
   if (err == cudaSuccess) err = b.alloc(&d_na, (size_t)Jall);
-  if (dos) {
-    std::vector<int> lut(256);
-    for (int c = 0; c < 256; c++)
-      lut[c] = h->code256[c] != h->code256[c] ? -1 : (int)nearbyint(h->dos_scale * h->code256[c]);
-    if (err == cudaSuccess) err = b.up(&d_lut, lut, s);
-  }
-  if (err != cudaSuccess) {
-    cudaGetLastError();
-    return fail(err == cudaErrorMemoryAllocation ? BSG_ERR_ALLOC : BSG_ERR_CUDA, "big_spLinReg scratch (%s)",
-                cudaGetErrorString(err));
-  }
-  Cols cs;
-  cs.P = dos ? h->dosV : h->A;
-  cs.stride = dos ? h->dosStride : h->strideA;
-  cs.D = dos ? (double)h->dos_scale : 0.0;
-  cs.rows = d_rows, cs.lines = d_cols, cs.cov = d_cov, cs.nr = nr, cs.G = nc;
+  if (err != cudaSuccess) return scratch_fail(err);
+  cs.cov = d_cov, cs.nr = nr, cs.G = nc;
   Events tm;
   BSG_CUDA(cudaEventCreate(&tm.ev[0]));
   BSG_CUDA(cudaEventCreate(&tm.ev[1]));
   BSG_CUDA(cudaEventRecord(tm.ev[0], s));
   if (Jall > 0) {
-    k_sp_stats<<<(Jall + ST / 32 - 1) / (ST / 32), ST, 0, s>>>(cs, Jall, h->raw, n, d_lut, d_ctr, d_sc, d_na);
+    k_sp_stats<<<(Jall + ST / 32 - 1) / (ST / 32), ST, 0, s>>>(cs, Jall, op.raw, n, op.lut, d_ctr, d_sc, d_na);
     count_launch();
     BSG_CUDA(cudaGetLastError());
   }
@@ -594,13 +712,12 @@ int bsg_splreg(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, int n
   BSG_CUDA(cudaMemcpyAsync(na.data(), d_na, (size_t)Jall, cudaMemcpyDeviceToHost, s));
   BSG_CUDA(cudaStreamSynchronize(s));
   for (int c = 0; c < nc; c++)
-    if (na[c])
-      return fail(BSG_ERR_ARG, "Column %d holds a missing value on a training row; impute it first "
-                               "(snp_fastImputeSimple).", ind_col ? ind_col[c] : c + 1);
+    if (na[c]) return fail(BSG_ERR_ARG, op.bad_msg, ind_col ? ind_col[c] : c + 1);
   for (int c = 0; c < Kc; c++)
     if (!(scale[nc + c] > SD_MIN)) return fail(BSG_ERR_ARG, "Covariate %d is constant over 'ind.train'.", c + 1);
-  // the fit's columns: kept genotype columns by line (ties in ind_col order), so that coordinate descent visits them in
-  // an order that does not depend on how ind_col is permuted, then the covariates; results go back in ind_col order
+  // the fit's columns: kept columns by index in the matrix (genotype line or dense column; ties in ind_col order), so
+  // that coordinate descent visits them in an order that does not depend on how ind_col is permuted, then the
+  // covariates; results go back in ind_col order
   std::vector<int> lines, ord;
   std::vector<double> fc, fis, fpf;
   for (int c = 0; c < nc; c++) {
@@ -609,7 +726,7 @@ int bsg_splreg(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, int n
   }
   std::stable_sort(ord.begin(), ord.end(), [&](int u, int v) { return col0[u] < col0[v]; });
   for (int c : ord) {
-    lines.push_back(col0[c]);
+    lines.push_back(op.line(c, col0));
     fc.push_back(center[c]);
     fis.push_back(1.0 / scale[c]);
     fpf.push_back(pf_X ? pf_X[c] : 1.0);
@@ -621,7 +738,7 @@ int bsg_splreg(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, int n
     fpf.push_back(pf_covar ? pf_covar[c] : 1.0);
   }
   if (J == 0) return fail(BSG_ERR_ARG, "No column varies over 'ind.train'.");
-  FArgs a;
+  FArgs<typename Op::Src> a;
   a.c = cs;
   a.c.G = G;
   a.J = J;
@@ -666,11 +783,7 @@ int bsg_splreg(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, int n
   if (err == cudaSuccess) err = b.alloc(&d_np, FL);
   if (err == cudaSuccess && path_beta) err = b.alloc(&d_pb, FL * J);
   if (err == cudaSuccess && path_b0) err = b.alloc(&d_pb0, FL);
-  if (err != cudaSuccess) {
-    cudaGetLastError();
-    return fail(err == cudaErrorMemoryAllocation ? BSG_ERR_ALLOC : BSG_ERR_CUDA, "big_spLinReg scratch (%s)",
-                cudaGetErrorString(err));
-  }
+  if (err != cudaSuccess) return scratch_fail(err);
   BSG_CUDA(cudaMemsetAsync(d_bb, 0, FJ * sizeof(double), s));
   BSG_CUDA(cudaMemsetAsync(d_b0, 0, (size_t)F * sizeof(double), s));
   BSG_CUDA(cudaMemsetAsync(d_lam, 0, FL * sizeof(double), s));
@@ -686,7 +799,8 @@ int bsg_splreg(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, int n
   a.r = d_r, a.w = d_w, a.s = d_s, a.beta = d_beta, a.z = d_z, a.v = d_v, a.flag = d_flag, a.wl = d_wl;
   a.bbest = d_bb, a.b0best = d_b0, a.best = d_best, a.len = d_len, a.msg = d_msg;
   a.lam = d_lam, a.loss = d_loss, a.nnz = d_nnz, a.npass = d_np, a.pbeta = d_pb, a.pb0 = d_pb0;
-  BSG_CUDA(cudaFuncSetAttribute(k_splreg, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Smem)));
+  BSG_CUDA(cudaFuncSetAttribute(k_splreg<typename Op::Src>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                (int)sizeof(Smem)));
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(F * CS);
   cfg.blockDim = dim3(ST);
@@ -697,7 +811,7 @@ int bsg_splreg(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, int n
   at[0].val.clusterDim.x = CS, at[0].val.clusterDim.y = 1, at[0].val.clusterDim.z = 1;
   cfg.attrs = at;
   cfg.numAttrs = 1;
-  BSG_CUDA(cudaLaunchKernelEx(&cfg, k_splreg, a));
+  BSG_CUDA(cudaLaunchKernelEx(&cfg, k_splreg<typename Op::Src>, a));
   count_launch();
   BSG_CUDA(cudaGetLastError());
   BSG_CUDA(cudaEventRecord(tm.ev[1], s));
@@ -733,6 +847,70 @@ int bsg_splreg(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, int n
   return BSG_OK;
 }
 
+}  // namespace splreg
+}  // namespace bsg
+
+using namespace bsg;
+
+extern "C" {
+
+int bsg_splreg(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, int nc, int family, const double *y,
+               const double *covar, int Kc, const double *base, const double *pf_X, const double *pf_covar,
+               const double *alphas, int nalpha, const int *ind_sets, int K, int nlambda, double lambda_min_ratio,
+               int nlam_min, int n_abort, int dfmax, double eps, int max_iter, double power_scale, double power_adaptive,
+               double *center, double *scale, uint8_t *kept, double *beta, double *intercept, int *best, int *length,
+               int *message, double *lambda, double *loss, int *nnz, int *npass, double *path_beta, double *path_b0) {
+  using namespace splreg;
+  if (!h) return fail(BSG_ERR_ARG, "null handle");
+  if (h->fbm_generic && !h->dos_scale)
+    return fail(BSG_ERR_TYPE, "big_spLinReg / big_spLogReg on the device need hard calls or dosages (codes multiples of "
+                              "1 / D); this FBM.code256 holds other values.");
+  BSG_TRY(bind_device(h));
+  BedOp op{h, h->n, h->m, h->stream, h->raw};
+  return splreg_drive(op, ind_row, nr, ind_col, nc, family, y, covar, Kc, base, pf_X, pf_covar, alphas, nalpha,
+                      ind_sets, K, nlambda, lambda_min_ratio, nlam_min, n_abort, dfmax, eps, max_iter, power_scale,
+                      power_adaptive, center, scale, kept, beta, intercept, best, length, message, lambda, loss, nnz,
+                      npass, path_beta, path_b0);
+}
+
+int bsg_splreg_dense(const void *X, int dtype, int64_t ld, int nrow, int ncol, const int *ind_row, int nr,
+                     const int *ind_col, int nc, int device, int family, const double *y, const double *covar, int Kc,
+                     const double *base, const double *pf_X, const double *pf_covar, const double *alphas, int nalpha,
+                     const int *ind_sets, int K, int nlambda, double lambda_min_ratio, int nlam_min, int n_abort,
+                     int dfmax, double eps, int max_iter, double power_scale, double power_adaptive, double *center,
+                     double *scale, uint8_t *kept, double *beta, double *intercept, int *best, int *length,
+                     int *message, double *lambda, double *loss, int *nnz, int *npass, double *path_beta,
+                     double *path_b0) {
+  using namespace splreg;
+  if (dtype != 0 && dtype != 1) return fail(BSG_ERR_TYPE, "dtype must be 0 (float) or 1 (double).");
+  if (nrow < 0 || ncol < 0 || ld < std::max(nrow, 1) || (!X && (int64_t)nrow * ncol > 0))
+    return fail(BSG_ERR_DIM, "Incompatibility between dimensions.");
+  if (cudaSetDevice(device) != cudaSuccess) {
+    cudaGetLastError();
+    return fail(BSG_ERR_CUDA, "CUDA device %d is not available (no CPU fallback).", device);
+  }
+  struct Stream {
+    cudaStream_t s = nullptr;
+    ~Stream() {
+      if (s) cudaStreamSynchronize(s), cudaStreamDestroy(s);
+    }
+  } st;
+  BSG_CUDA(cudaStreamCreateWithFlags(&st.s, cudaStreamNonBlocking));
+#define BSG_SPLREG_TAIL                                                                                                  \
+  ind_row, nr, ind_col, nc, family, y, covar, Kc, base, pf_X, pf_covar, alphas, nalpha, ind_sets, K, nlambda,           \
+      lambda_min_ratio, nlam_min, n_abort, dfmax, eps, max_iter, power_scale, power_adaptive, center, scale, kept, beta, \
+      intercept, best, length, message, lambda, loss, nnz, npass, path_beta, path_b0
+  if (dtype == 0) {
+    DenseOp<float> op{static_cast<const float *>(X), ld, nrow, ncol, st.s};
+    return splreg_drive(op, BSG_SPLREG_TAIL);
+  }
+  DenseOp<double> op{static_cast<const double *>(X), ld, nrow, ncol, st.s};
+  return splreg_drive(op, BSG_SPLREG_TAIL);
+#undef BSG_SPLREG_TAIL
+}
+
 double bsg_splreg_last_ms(void) { return splreg::g_last_ms; }
+
+double bsg_splreg_last_stage_ms(void) { return splreg::g_stage_ms; }
 
 }  // extern "C"

@@ -323,8 +323,28 @@ int bsg_splreg(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, int n
                int nlam_min, int n_abort, int dfmax, double eps, int max_iter, double power_scale, double power_adaptive,
                double *center, double *scale, uint8_t *kept, double *beta, double *intercept, int *best, int *length,
                int *message, double *lambda, double *loss, int *nnz, int *npass, double *path_beta, double *path_b0);
-/* device time in ms (CUDA events) of the last bsg_splreg: column statistics to the end of the last fit */
+/* bsg_splreg over a dense host matrix instead of a handle: X is column-major with leading dimension ld >= nrow, nrow x ncol
+ * elements of float (dtype 0) or double (dtype 1); ind_row / ind_col index it (1-based, repeats allowed, NULL = all).
+ * X[ind_row, ind_col] is gathered through bounded pinned buffers and uploaded once to `device` (nr x nc elements of the
+ * same type); each element is widened to double exactly when read, so the fit is bsg_splreg's on X converted to double:
+ * same arguments after ind_col, same outputs, same arithmetic and summation order.  Coordinate descent visits the kept
+ * columns by increasing column index (ties in ind_col order), then the covariates.  Refusals: those of bsg_splreg; a
+ * dtype other than 0 / 1: BSG_ERR_TYPE; ld < nrow, negative sizes or a null X: BSG_ERR_DIM; a non-finite value on a
+ * selected (row, column) pair: BSG_ERR_ARG naming the column, after the column-statistics pass; the staged block plus the
+ * fits' state beyond free device memory: BSG_ERR_ALLOC with the bytes needed, before any allocation. */
+int bsg_splreg_dense(const void *X, int dtype, int64_t ld, int nrow, int ncol, const int *ind_row, int nr,
+                     const int *ind_col, int nc, int device, int family, const double *y, const double *covar, int Kc,
+                     const double *base, const double *pf_X, const double *pf_covar, const double *alphas, int nalpha,
+                     const int *ind_sets, int K, int nlambda, double lambda_min_ratio, int nlam_min, int n_abort,
+                     int dfmax, double eps, int max_iter, double power_scale, double power_adaptive, double *center,
+                     double *scale, uint8_t *kept, double *beta, double *intercept, int *best, int *length,
+                     int *message, double *lambda, double *loss, int *nnz, int *npass, double *path_beta,
+                     double *path_b0);
+/* device time in ms (CUDA events) of the last bsg_splreg / bsg_splreg_dense: column statistics to the end of the last
+ * fit */
 double bsg_splreg_last_ms(void);
+/* host time in ms of the last call's staging: the dense gather and upload, or the dosage value copy when it is built */
+double bsg_splreg_last_stage_ms(void);
 
 /* ---- sparse LD matrix (bigsparser's SFBM) and summary-statistics PRS -------------------------------------- */
 /* as_SFBM(corr[, compact]) staged to HBM once, in bigsparser's storage as bigsnpr reads it (src/ld-scores-sfbm.cpp:14-66):
