@@ -40,6 +40,24 @@ Where nvcc contracts a multiply and an add, the model does the same.  `cuobjdump
 The fused slice-0 multiply and the split scalbn only change a result whose scaled slice totals are subnormal (vectors
 of subnormal size); in every other range the products by powers of two are exact.
 
+Dosage FBM.code256 handles (bsg_dosage.cu, `dosage_*`) share the vector side: X.y takes prep_T's digits (hb = 0, one
+digit block per selected column), Xt.y k_prep1 + k_quantise's scatter by physical sample (hb_bits(row multiplicity)).
+The matrix operand is q = nearbyint(D code256[b]) in 0..255 (an NA byte counts 0), so |digit x q| <= 32,640 and a
+k-split of 65,536 contraction indices stays within int32; the partials are exact integers as above.  The same SASS shows:
+  * k_finish_dprod: every slice of the combine is DMUL + DADD, slice 0 included (`/*1970*/ DADD R8, R8, R10`): no fused
+    last slice (combine(..., fused0=False)); then the IEEE division by D; C summed by DADD from 0.0 in block order; and
+    `/*2ad0*/ DADD R8, -R8, R2`: full = R / D - C;
+  * k_finish_dcprod: the same combine (`/*1940*/ DADD R8, R8, R10`), R / D, then `/*20f0*/ DFMA R8, -R2, R8, R6`:
+    out = fma(-c, Y, R / D), divided by s;
+  * k_lit_prod: `/*07d0*/ DFMA R28, R30, R10, R28`: s = fma(x_t, (code256[b] - c_t) / s_t, s);
+  * k_lit_cprod: `/*0700*/ DFMA R16, R16, R12, RZ` then `/*0950*/ DFMA R16, R10, R12, R16`: lane sums by fma, then the
+    butterfly by DADD (`/*2730*/ DADD R10, R10, R16`);
+  * k_proj_literal<false> / <true>: `/*06c0*/ DFMA R12, R16, R16, R12` / `/*0660*/ DFMA R14, R16, R16, R14`:
+    rss = fma(x, x, rss); `/*08d0*/ DFMA R18, R20, R16, R18` / `/*0870*/ DFMA R18, R20, R16, R18`: XV = fma(V, x, XV).
+    x = (v - c) / s is a DADD and an IEEE division (MUFU.RCP64H, DFMA refinement, slow-path CALL) in every literal loop.
+(Offsets within each function of `cuobjdump -sass libbsgpu.so`.)  Accuracy of X.y: |out - exact| <= sum_t (q_t / D)
+|z_t| ... as above with g = q / D: 2^(-e-1) sum_t q_t / D + a few ulps of |out| + the rounding of 1 / D and of C.
+
 Accuracy this proves (one vector, 61-bit format): |out - exact| <= sum_t |g_t| 2^(-e-1) (quantisation, g the
 codes or scaled codes the vector meets) + a few ulps of |out| (combine) + the rounding of C.  e = 60 - ex - hb with
 max |v| < 2^ex, so the quantisation term is below 2^(-61+hb) max|v| sum_t |g_t|: about 4e-19 max|v| sum|g| without
@@ -79,8 +97,19 @@ def pick_e(m: float, hb: int, bits: int) -> int:
 
 
 def fma(a: float, b: float, c: float) -> float:
-    """a * b + c rounded once (Fraction arithmetic; int / int true division is correctly rounded)."""
-    return float(Fraction(a) * Fraction(b) + Fraction(c))
+    """a * b + c rounded once (Fraction arithmetic; int / int true division is correctly rounded).  Non-finite operands
+    give what the fp64 ops give; an exact zero keeps IEEE's sign (+0 from a cancellation, the signed sum when a b = 0);
+    an overflow is an infinity."""
+    a, b, c = float(a), float(b), float(c)
+    if not (math.isfinite(a) and math.isfinite(b) and math.isfinite(c)):
+        return a * b + c
+    r = Fraction(a) * Fraction(b) + Fraction(c)
+    if r == 0:
+        return a * b + c if (a == 0.0 or b == 0.0) else 0.0
+    try:
+        return float(r)
+    except OverflowError:
+        return math.copysign(math.inf, r)
 
 
 # ---- vector preparation ---------------------------------------------------------------------------------------------
@@ -193,8 +222,9 @@ def _add_scaled(acc: np.ndarray, v: np.ndarray, k: int, fused: bool) -> np.ndarr
     return np.array([_add_scaled1(float(a), int(x), k, fused) for a, x in zip(acc, v)])
 
 
-def combine(raw, na, c0: int, c1: int, e: int, ns: int = 8, s0: int = 0) -> np.ndarray:
-    """combine<NS>: sum over s = NS-1 .. 0 of scalbn(c0 raw[s0+s] + c1 na[s0+s], 8 s - e), top down."""
+def combine(raw, na, c0: int, c1: int, e: int, ns: int = 8, s0: int = 0, fused0: bool = True) -> np.ndarray:
+    """combine<NS>: sum over s = NS-1 .. 0 of scalbn(c0 raw[s0+s] + c1 na[s0+s], 8 s - e), top down.  fused0: the last
+    slice's multiply is fused with its add (the 2-bit finish kernels; the dosage ones keep DMUL + DADD)."""
     raw = np.asarray(raw, dtype=np.int64)
     na = np.zeros_like(raw) if na is None else np.asarray(na, dtype=np.int64)
     acc = np.zeros(raw.shape[0])
@@ -204,7 +234,7 @@ def combine(raw, na, c0: int, c1: int, e: int, ns: int = 8, s0: int = 0) -> np.n
             v = v + c0 * raw[:, s0 + s]
         if c1:
             v = v + c1 * na[:, s0 + s]
-        acc = _add_scaled(acc, v, 8 * s - e, fused=s == 0)
+        acc = _add_scaled(acc, v, 8 * s - e, fused=fused0 and s == 0)
     return acc
 
 
@@ -431,6 +461,179 @@ def row_sums_sq(G, ir, iy, center, scale, pmv=False):
         _, N = _plane_sums(Gl, c0, m, nv, nv, "na", pmv)
         t2 = (-N) + 0.0
     return ((t1 + t2) + T)[r0]
+
+
+# ---- dosage FBM.code256 (bsg_dosage.cu) -------------------------------------------------------------------------------
+def dosage_table(code256):
+    """dosage_scale_of: the smallest D in 1..255 with D v within 1e-9 of an integer in 0..255 for every non-NaN v of the
+    table (0 when none, or when an entry is infinite); the byte map q = nearbyint(D v) (NA -> 0) of the value copy; the NA
+    flags.  Returns (D, q, na); q is None when D = 0."""
+    code = np.asarray(code256, dtype=np.float64)
+    na = np.isnan(code)
+    v = code[~na]
+    if not np.all(np.isfinite(v)):
+        return 0, None, na
+    for D in range(1, 256):
+        t = D * v
+        r = np.rint(t)
+        if np.all((np.abs(t - r) <= 1e-9) & (r >= 0) & (r <= 255)):
+            q = np.where(na, 0.0, np.rint(D * np.where(na, 0.0, code))).astype(np.uint8)
+            return D, q, na
+    return 0, None, na
+
+
+def _dsel(raw, ir, ic):
+    raw = np.asarray(raw, dtype=np.uint8)
+    n, m = raw.shape
+    r0 = np.arange(n) if ir is None else np.asarray(ir, dtype=np.int64) - 1
+    c0 = np.arange(m) if ic is None else np.asarray(ic, dtype=np.int64) - 1
+    return raw, r0, c0
+
+
+def dosage_prod(raw, code256, ir, ic, y, center=None, scale=None):
+    """X.y on a dosage handle (dosage_prep_cols -> prep_T, k_dmvT, k_finish_dprod, k_na_rows, k_gather_rows).
+
+    Lines are the selected columns in selection order, each with its own digits of z = y / s (or y), so hb = 0; the
+    contraction runs over q[byte] of the value copy (an NA byte counts 0); R = combine<8> of the slice totals, then R / D,
+    then - C with scaling.  Every sample holding an NA byte in a selected column is NaN, then the rows are gathered.  A
+    non-finite z or (c - 3) z (k_prep1's flag) makes every output NaN (the device-pointer forms; the host forms re-run
+    `lit_prod` instead)."""
+    D, qmap, isna = dosage_table(code256)
+    raw, r0, c0 = _dsel(raw, ir, ic)
+    c, s = _scaling(center, scale)
+    scaled = c is not None
+    with np.errstate(all="ignore"):
+        v0, v1 = make_vals(1 if scaled else 0, y, c, s)
+    if not (np.all(np.isfinite(v0)) and np.all(np.isfinite(v1))):
+        return np.full(r0.size, np.nan)
+    e = pick_e(float(np.max(np.abs(v0), initial=0.0)), 0, 60)
+    part = partials(qmap[raw[:, c0]], digits(quantise(v0, e), 8))
+    full = combine(part, None, 1, 0, e, fused0=False) / D
+    if scaled:
+        full = full - sum_cz(c, v0)
+    full[isna[raw[:, c0]].any(axis=1)] = np.nan
+    return full[r0]
+
+
+def dosage_cprod(raw, code256, ir, ic, y, center=None, scale=None):
+    """Xt.y on a dosage handle (dosage_prep_rows -> k_prep1 + k_quantise, k_digits_rows, k_dmv, k_finish_dcprod,
+    k_na_lines / k_na_cols).
+
+    y is quantised with hb_bits(row multiplicity) and scattered by physical sample; lines are the selected columns, the
+    contraction runs over all n samples of the value copy; R = combine<8> / D; with scaling out = fma(-c, Y, R) / s with
+    Y = scalbn(sum_hi, 32 - e) + scalbn(sum_lo, -e) from the exact sum of Q.  A line holding an NA byte in a selected row
+    is NaN.  A non-finite y, center or 1 / scale makes every output NaN (k_check_scaling)."""
+    D, qmap, isna = dosage_table(code256)
+    raw, r0, c0 = _dsel(raw, ir, ic)
+    n = raw.shape[0]
+    c, s = _scaling(center, scale)
+    y = np.asarray(y, dtype=np.float64)
+    with np.errstate(all="ignore"):
+        bad = not np.all(np.isfinite(y)) or (c is not None and not (np.all(np.isfinite(c)) and np.all(np.isfinite(1.0 / s))))
+    if bad:
+        return np.full(c0.size, np.nan)
+    e = pick_e(float(np.max(np.abs(y), initial=0.0)), hb_bits(max_mult(r0)), 60)
+    q = scatter(quantise(y, e), r0, n)
+    part = partials(qmap[raw[:, c0]].T, digits(q, 8))
+    R = combine(part, None, 1, 0, e, fused0=False) / D
+    if c is None:
+        out = R
+    else:
+        sum_hi, sum_lo = int(np.sum(q >> 32)), int(np.sum(q & _M32))
+        Y = math.ldexp(float(sum_hi), 32 - e) + math.ldexp(float(sum_lo), -e)
+        out = np.array([fma(-cj, Y, Rj) for cj, Rj in zip(c, R)]) / s
+    rows = np.unique(r0)
+    out[isna[raw[np.ix_(rows, c0)]].any(axis=0)] = np.nan
+    return out
+
+
+def _lit_terms(code, raw, r0, col, cj, sj):
+    """(code256[b] - c) / s for the bytes of one column at rows r0 (one IEEE subtraction and division each)."""
+    with np.errstate(all="ignore"):
+        return (np.asarray(code, dtype=np.float64)[raw[r0, col]] - cj) / sj
+
+
+def _fma_vec(a, b, c):
+    a, b, c = np.broadcast_arrays(np.asarray(a, dtype=np.float64), np.asarray(b, dtype=np.float64),
+                                  np.asarray(c, dtype=np.float64))
+    return np.array([fma(x, y, z) for x, y, z in zip(a.ravel(), b.ravel(), c.ravel())]).reshape(a.shape)
+
+
+def _lit_scaling(center, scale, nc):
+    c, s = _scaling(center, scale)
+    return (np.zeros(nc), np.ones(nc)) if c is None else (c, s)
+
+
+def lit_prod(raw, code256, ir, ic, x, center=None, scale=None):
+    """k_lit_prod: one thread per selected row, a serial loop over the selected columns in order,
+    s = fma(x_t, (code256[b] - c_t) / s_t, s) from 0 (non-finite values propagate as in fp64)."""
+    raw, r0, c0 = _dsel(raw, ir, ic)
+    c, s = _lit_scaling(center, scale, c0.size)
+    x = np.asarray(x, dtype=np.float64)
+    acc = np.zeros(r0.size)
+    for t in range(c0.size):
+        acc = _fma_vec(_lit_terms(code256, raw, r0, c0[t], c[t], s[t]), x[t], acc)
+    return acc
+
+
+def lit_cprod(raw, code256, ir, ic, x, center=None, scale=None):
+    """k_lit_cprod: one warp per selected column; lane l sums rows l, l + 32, ... with s = fma(term, x_i, s) from 0,
+    then the xor butterfly 16, 8, 4, 2, 1 (DADD) and lane 0's value."""
+    raw, r0, c0 = _dsel(raw, ir, ic)
+    c, s = _lit_scaling(center, scale, c0.size)
+    x = np.asarray(x, dtype=np.float64)
+    nr = r0.size
+    out = np.empty(c0.size)
+    for t in range(c0.size):
+        term = _lit_terms(code256, raw, r0, c0[t], c[t], s[t])
+        lanes = np.zeros(32)
+        for i0 in range(0, nr, 32):
+            k = min(32, nr - i0)
+            lanes[:k] = _fma_vec(term[i0:i0 + k], x[i0:i0 + k], lanes[:k])
+        idx = np.arange(32)
+        with np.errstate(all="ignore"):
+            for o in (16, 8, 4, 2, 1):
+                lanes = lanes + lanes[idx ^ o]
+        out[t] = lanes[0]
+    return out
+
+
+def proj_literal(P, code256, ir, ic, center, scale, V=None):
+    """k_proj_literal<BYTES> (prod_and_rowSumsSq2's literal pass): one thread per selected row, a serial loop over the
+    selected columns in order.  code256 given: P is the n x m code bytes, v = code256[b]; code256 None: P holds hard calls
+    0 / 1 / 2 / 3 (3 = NA -> NaN).  x = (v - c) / s, rss = fma(x, x, rss), XV[:, k] = fma(V[j, k], x, XV[:, k]) from 0.
+    Returns (XV, rss, na) with na = the rows where a selected column holds an NA."""
+    P, r0, c0 = _dsel(P, ir, ic)
+    c, s = _lit_scaling(center, scale, c0.size)
+    code = np.r_[0.0, 1.0, 2.0, np.nan] if code256 is None else np.asarray(code256, dtype=np.float64)
+    V = np.zeros((c0.size, 0)) if V is None else np.asarray(V, dtype=np.float64).reshape(c0.size, -1)
+    rss, XV = np.zeros(r0.size), np.zeros((r0.size, V.shape[1]))
+    na = np.zeros(r0.size, dtype=bool)
+    for j in range(c0.size):
+        x = _lit_terms(code, P, r0, c0[j], c[j], s[j])
+        na |= np.isnan(code[P[r0, c0[j]]])
+        rss = _fma_vec(x, x, rss)
+        for k in range(V.shape[1]):
+            XV[:, k] = _fma_vec(V[j, k], x, XV[:, k])
+    return XV, rss, na
+
+
+def exact_dosage_prod(raw, code256, ir, ic, y, center=None, scale=None):
+    """X~ y over a dosage table in rationals: sum over the selected columns of (q / D - c) / s y; None where an NA byte
+    meets the row."""
+    D, qmap, isna = dosage_table(code256)
+    raw, r0, c0 = _dsel(raw, ir, ic)
+    c, s = _lit_scaling(center, scale, c0.size)
+    w = [Fraction(float(yk)) / Fraction(float(sk)) for yk, sk in zip(y, s)]
+    out = []
+    for i in r0:
+        b = raw[i, c0]
+        if isna[b].any():
+            out.append(None)
+            continue
+        out.append(sum(((Fraction(int(qmap[bb]), D) - Fraction(float(c[t]))) * w[t] for t, bb in enumerate(b)),
+                       Fraction(0)))
+    return out
 
 
 # ---- exact references -------------------------------------------------------------------------------------------------

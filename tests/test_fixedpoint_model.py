@@ -194,3 +194,152 @@ def test_head_room_covers_rounding_up_to_the_binade():
         yy = np.full(mult, np.nextafter(1.0, 0.0))
         tot = int(fx.scatter(fx.quantise(yy, fx.pick_e(yy[0], fx.hb_bits(mult), 60)), np.zeros(mult, int), 1)[0])
         assert 0 < tot < 2 ** 60 and 8 * tot < 2 ** 63
+
+
+# ---- dosage FBM.code256 (bsg_dosage.cu) -------------------------------------------------------------------------------
+CODE_DOSAGE = np.concatenate([[0, 1, 2, np.nan, 0, 1, 2], np.arange(201) * 0.01, np.full(48, np.nan)])
+
+
+def dosage_tables():
+    """Tables of every scale the dosage kernels serve: CODE_DOSAGE (D = 100), bytes as values (D = 1, up to 255), k / 255
+    (D = 255, byte 255 -> q = 255), and D = 4 / D = 2 tables holding NA entries."""
+    d4 = np.arange(256) / 4.0
+    d4[[3, 77, 200]] = np.nan
+    d2 = np.arange(256) / 2.0
+    d2[[5, 254]] = np.nan
+    return {"dosage": (CODE_DOSAGE, 100), "d1": (np.arange(256.0), 1), "d255": (np.arange(256) / 255.0, 255),
+            "d4": (d4, 4), "d2": (d2, 2)}
+
+
+def worst_case_vector(k, e=60):
+    """k copies of y = Q 2^-e with Q = -(9 2^56 + sum_{s<7} 128 256^s): digits -128 in slices 0..6 and -9 in slice 7."""
+    Q = -(9 * 2 ** 56 + sum(128 * 256 ** s for s in range(7)))
+    return np.full(k, math.ldexp(float(Q), -e)), Q
+
+
+def test_dosage_table_rule():
+    for name, (code, D) in dosage_tables().items():
+        got, q, na = fx.dosage_table(code)
+        assert got == D, name
+        ok = ~np.isnan(code)
+        assert np.array_equal(na, ~ok) and np.all(q[~ok] == 0)
+        assert np.array_equal(q[ok].astype(float), np.rint(D * code[ok])) and np.max(q) <= 255
+    D, q, na = fx.dosage_table(CODE_DOSAGE)
+    assert list(q[:7]) == [0, 100, 200, 0, 0, 100, 200] and q[7 + 137] == 137 and q[207] == 200 and na[3] and na[230]
+    assert fx.dosage_table(np.linspace(0, 2, 256))[0] == 0                     # no D makes every value an integer
+    assert fx.dosage_table(np.r_[np.inf, np.arange(255.0)])[0] == 0           # an infinite entry
+    assert fx.dosage_table(np.r_[256.0, np.arange(255.0)])[0] == 0            # q would exceed 255
+    assert fx.dosage_table(np.arange(256) / 255.0)[1][255] == 255
+
+
+def _dosage_bound(Dq, ir, ic, y, center, scale, D, hb=0, cprod=False):
+    """Quantisation + combine + 1 / D + C bound of one dosage product (as the 2-bit model's bound): each vector entry is
+    off by at most 2^(-e-1) after rint, and meets q / D in every value of its line."""
+    n, m = Dq.shape
+    r0 = np.arange(n) if ir is None else ir - 1
+    c0 = np.arange(m) if ic is None else ic - 1
+    c = np.zeros(c0.size) if center is None else np.asarray(center)
+    s = np.ones(c0.size) if scale is None else np.asarray(scale)
+    val = Dq[np.ix_(r0, c0)] / D
+    if not cprod:
+        v = np.asarray(y) / s
+        e = fx.pick_e(float(np.max(np.abs(v))), 0, 60)
+        quant = val.sum(1) * 2.0 ** (-e - 1)
+        mag = ((val + np.abs(c)) * np.abs(v)).sum(1) + np.abs(c * v).sum()
+    else:
+        e = fx.pick_e(float(np.max(np.abs(y))), hb, 60)
+        quant = ((val + np.abs(c)) / s).sum(0) * 2.0 ** (-e - 1)
+        mag = ((val + np.abs(c)) / s * np.abs(np.asarray(y))[:, None]).sum(0)
+    return quant + 8 * 2.0 ** -52 * mag + 1e-300
+
+
+@pytest.mark.parametrize("table", ["dosage", "d1", "d255", "d4", "d2"])
+@pytest.mark.parametrize("scaled", [False, True])
+def test_dosage_model_within_its_bound_of_the_exact_product(rng, table, scaled):
+    code, D = dosage_tables()[table]
+    n, m = 29, 43
+    raw = rng.integers(0, 256, size=(n, m)).astype(np.uint8)
+    _, qmap, isna = fx.dosage_table(code)
+    ic = np.r_[np.repeat(rng.choice(m, 2, replace=False) + 1, 5), rng.integers(1, m + 1, 20)]   # a multiset
+    ir = np.r_[np.repeat(rng.choice(n, 2, replace=False) + 1, 17), rng.integers(1, n + 1, 12)]
+    c, s = (rng.uniform(0, 2, size=ic.size), rng.uniform(0.3, 2.0, size=ic.size)) if scaled else (None, None)
+    y = rng.normal(size=ic.size)
+    got = fx.dosage_prod(raw, code, None, ic, y, c, s)
+    exact = fx.exact_dosage_prod(raw, code, None, ic, y, c, s)
+    hit = np.array([w is None for w in exact])
+    assert np.array_equal(np.isnan(got), hit) and (not isna.any() or hit.any())
+    bound = _dosage_bound(qmap[raw].astype(float), None, ic, y, c, s, D)
+    for a, w, b in zip(got, exact, bound):
+        assert w is None or abs(Fraction(float(a)) - w) <= b
+    # Xt.y: the exact product over the transposed selection, NaN on the lines an NA byte meets
+    yr = rng.normal(size=ir.size)
+    cc = None if c is None else rng.uniform(0, 2, size=ic.size)
+    got = fx.dosage_cprod(raw, code, ir, ic, yr, cc, s)
+    cz = np.zeros(ic.size) if cc is None else cc
+    sz = np.ones(ic.size) if s is None else s
+    bound = _dosage_bound(qmap[raw].astype(float), ir, ic, yr, cc, s, D, fx.hb_bits(fx.max_mult(ir - 1)), cprod=True)
+    for t, j in enumerate(ic - 1):
+        b = raw[ir - 1, j]
+        if isna[b].any():
+            assert np.isnan(got[t])
+            continue
+        w = sum(((Fraction(int(qmap[bb]), D) - Fraction(float(cz[t]))) / Fraction(float(sz[t])) * Fraction(float(yy))
+                 for bb, yy in zip(b, yr)), Fraction(0))
+        assert abs(Fraction(float(got[t])) - w) <= bound[t]
+
+
+def test_worst_case_vector_reaches_the_int32_cap():
+    """The vector that drives every digit slice to -128: |Q| in [2^59, 2^60), set bits 7..59 (an exact double), so
+    pick_e returns e; 65,536 lines of q = 255 put -2,139,095,040 in each accumulator, 65,794 lines would pass -2^31."""
+    y, Q = worst_case_vector(4)
+    assert 2 ** 59 <= -Q < 2 ** 60 and int(math.ldexp(y[0], 60)) == Q
+    assert fx.pick_e(float(np.max(np.abs(y))), 0, 60) == 60
+    q = fx.quantise(y, 60)
+    assert np.all(q == Q)
+    d = fx.digits(q, 8)
+    assert np.all(d[:, :7] == -128) and np.all(d[:, 7] == -9)
+    one = fx.partials(np.full((1, 1), 255), d[:1])[0]
+    assert np.all(one[:7] * 65536 == -2139095040) and -2139095040 >= -(2 ** 31)
+    assert one[0] * 65793 >= -(2 ** 31) > one[0] * 65794
+
+
+def test_literal_models_within_rounding_of_the_exact_sums(rng):
+    """lit_prod / lit_cprod / proj_literal against rationals (finite input) and fp64 NumPy (NaN / Inf pattern)."""
+    n, m = 45, 37
+    raw = rng.integers(0, 208, size=(n, m)).astype(np.uint8)
+    raw[rng.random((n, m)) < 0.01] = 230
+    raw[0, :] = 3
+    ir, ic = rng.integers(1, n + 1, 40), rng.integers(1, m + 1, 35)
+    c, s = rng.uniform(0, 2, size=35), rng.uniform(0.3, 2.0, size=35)
+    x, yr = rng.normal(size=35), rng.normal(size=40)
+    X = (CODE_DOSAGE[raw[np.ix_(ir - 1, ic - 1)]] - c) / s
+    ok = ~np.isnan(X)
+    for got, want, mag in ((fx.lit_prod(raw, CODE_DOSAGE, ir, ic, x, c, s), X @ x, np.abs(X) @ np.abs(x)),
+                           (fx.lit_cprod(raw, CODE_DOSAGE, ir, ic, yr, c, s), yr @ X, np.abs(yr) @ np.abs(X))):
+        assert np.array_equal(np.isnan(got), np.isnan(want)) and np.isnan(want).any()
+        fin = ~np.isnan(want)
+        assert np.all(np.abs(got[fin] - want[fin]) <= 64 * 2.0 ** -52 * mag[fin])
+    V = rng.normal(size=(35, 2))
+    XV, rss, na = fx.proj_literal(raw, CODE_DOSAGE, ir, ic, c, s, V)
+    assert np.array_equal(na, ~ok.all(axis=1)) and np.array_equal(np.isnan(rss), na)
+    Xz = np.where(ok, X, 0.0)
+    assert np.all(np.abs(rss[~na] - (Xz * Xz).sum(1)[~na]) <= 64 * 2.0 ** -52 * (Xz * Xz).sum(1)[~na])
+    assert np.allclose(XV[~na], (Xz @ V)[~na], rtol=0, atol=1e-12)
+    # exact in rationals for one row: the serial fma loop rounds once per column
+    i = int(np.nonzero(~na)[0][0])
+    acc = 0.0
+    for j in range(35):
+        acc = float(Fraction(float(X[i, j])) * Fraction(float(X[i, j])) + Fraction(acc))
+    assert rss[i] == acc
+    # non-finite input: Inf / NaN propagate as in fp64
+    s0 = s.copy()
+    s0[3] = 0.0
+    with np.errstate(all="ignore"):
+        want = (((CODE_DOSAGE[raw[np.ix_(ir - 1, ic - 1)]] - c) / s0) * x).sum(1)  # one infinite column
+    got = fx.lit_prod(raw, CODE_DOSAGE, ir, ic, x, c, s0)
+    assert np.array_equal(np.isinf(got), np.isinf(want)) and np.array_equal(np.isnan(got), np.isnan(want))
+    assert np.isinf(got).any() and np.all(got[np.isfinite(want)] == want[np.isfinite(want)])
+    # hard calls: code 3 is NA
+    G = rng.integers(0, 4, size=(n, m)).astype(np.uint8)
+    XV, rss, na = fx.proj_literal(G, None, ir, ic, c, s, V)
+    assert np.array_equal(na, (G[np.ix_(ir - 1, ic - 1)] == 3).any(axis=1)) and np.array_equal(np.isnan(XV[:, 0]), na)
