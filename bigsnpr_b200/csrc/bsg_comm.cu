@@ -384,11 +384,12 @@ static int group_views(bsg_group *g, const int *ind_row, int nr, const int *ind_
       g->pos[i].clear();
     }
     if (ind_col) {
+      std::vector<int> col0;
+      BSG_TRY(host_index(ind_col, nc, g->m, "column ", col0));
       for (int t = 0; t < nc; t++) {
-        const long long c = (long long)ind_col[t] - 1;
-        if (c < 0 || c >= g->m) return fail(BSG_ERR_BOUNDS, "Tested subscript out of bounds (column %d not in 1..%d).", ind_col[t], g->m);
-        const int own = (int)(std::upper_bound(g->col0.begin(), g->col0.begin() + g->ndev, (int)c) - g->col0.begin()) - 1;
-        g->loc[own].push_back((int)c - g->col0[own] + 1);
+        const int c = col0[t];
+        const int own = (int)(std::upper_bound(g->col0.begin(), g->col0.begin() + g->ndev, c) - g->col0.begin()) - 1;
+        g->loc[own].push_back(c - g->col0[own] + 1);
         g->pos[own].push_back(t);
       }
     } else {
@@ -639,11 +640,12 @@ int bsg_group_randomsvd(bsg_group *g, const int *ind_row, int nr, const int *ind
   if ((center == nullptr) != (scale == nullptr)) return fail(BSG_ERR_ARG, "center and scale must be given together");
   // bucket the columns (same rule as group_views, without building product views: the driver owns its own)
   std::vector<std::vector<int>> loc(g->ndev), pos(g->ndev);
+  std::vector<int> col0;
+  BSG_TRY(host_index(ind_col, nc, g->m, "column ", col0));
   for (int t = 0; t < nc; t++) {
-    const long long c = ind_col ? (long long)ind_col[t] - 1 : t;
-    if (c < 0 || c >= g->m) return fail(BSG_ERR_BOUNDS, "Tested subscript out of bounds (column %d not in 1..%d).", ind_col[t], g->m);
-    const int own = (int)(std::upper_bound(g->col0.begin(), g->col0.begin() + g->ndev, (int)c) - g->col0.begin()) - 1;
-    loc[own].push_back((int)c - g->col0[own] + 1);
+    const int c = col0[t];
+    const int own = (int)(std::upper_bound(g->col0.begin(), g->col0.begin() + g->ndev, c) - g->col0.begin()) - 1;
+    loc[own].push_back(c - g->col0[own] + 1);
     pos[own].push_back(t);
   }
   std::vector<std::vector<double>> cs(g->ndev), ss(g->ndev);
@@ -677,11 +679,12 @@ int bsg_group_tcrossprod(bsg_group *g, const int *ind_row, int nr, const int *in
   if (!ind_col) nc = g->m;
   std::vector<std::vector<int>> loc(g->ndev);
   std::vector<std::vector<double>> cs(g->ndev), ss(g->ndev);
+  std::vector<int> col0;
+  BSG_TRY(host_index(ind_col, nc, g->m, "column ", col0));
   for (int t = 0; t < nc; t++) {
-    const long long c = ind_col ? (long long)ind_col[t] - 1 : t;
-    if (c < 0 || c >= g->m) return fail(BSG_ERR_BOUNDS, "Tested subscript out of bounds (column %d not in 1..%d).", ind_col[t], g->m);
-    const int own = (int)(std::upper_bound(g->col0.begin(), g->col0.begin() + g->ndev, (int)c) - g->col0.begin()) - 1;
-    loc[own].push_back((int)c - g->col0[own] + 1);
+    const int c = col0[t];
+    const int own = (int)(std::upper_bound(g->col0.begin(), g->col0.begin() + g->ndev, c) - g->col0.begin()) - 1;
+    loc[own].push_back(c - g->col0[own] + 1);
     cs[own].push_back(center[t]);
     ss[own].push_back(scale[t]);
   }

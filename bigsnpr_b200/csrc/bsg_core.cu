@@ -437,20 +437,100 @@ int build_copy_B(bsg_bed *h) {
   return BSG_OK;
 }
 
+int alloc_fail(cudaError_t e, const char *what) {
+  cudaGetLastError();
+  return fail(e == cudaErrorMemoryAllocation ? BSG_ERR_ALLOC : BSG_ERR_CUDA, "%s (%s)", what, cudaGetErrorString(e));
+}
+
+cudaError_t CallTimer::start(cudaStream_t s) {
+  for (cudaEvent_t &e : ev)
+    if (!e) {
+      const cudaError_t c = cudaEventCreate(&e);
+      if (c != cudaSuccess) return c;
+    }
+  return cudaEventRecord(ev[0], s);
+}
+
+cudaError_t CallTimer::stop(cudaStream_t s) { return cudaEventRecord(ev[1], s); }
+
+cudaError_t CallTimer::elapsed(float *ms) const {
+  if (!ev[1]) return cudaErrorNotReady;
+  const cudaError_t e = cudaEventSynchronize(ev[1]);
+  return e != cudaSuccess ? e : cudaEventElapsedTime(ms, ev[0], ev[1]);
+}
+
+// largest number of times one value of z (all in [0, limit)) occurs: counted by value when z covers a good part of
+// the range, else over a sorted copy, so a short index into a large range costs O(len log len), not O(limit)
+static int max_mult(const std::vector<int> &z, int limit) {
+  int best = 1;
+  if ((int64_t)z.size() * 4 >= limit) {
+    std::vector<int> cnt(limit, 0);
+    for (int v : z) best = std::max(best, ++cnt[v]);
+    return best;
+  }
+  std::vector<int> s(z);
+  std::sort(s.begin(), s.end());
+  for (size_t i = 1, run = 1; i < s.size(); i++) {
+    run = s[i] == s[i - 1] ? run + 1 : 1;
+    best = std::max(best, (int)run);
+  }
+  return best;
+}
+
+int host_index(const int *ind, int len, int limit, const char *label, std::vector<int> &out, int *maxmult) {
+  out.resize(len > 0 ? len : 0);
+  for (int i = 0; i < len; i++) {
+    const long long v = ind ? (long long)ind[i] - 1 : i;
+    if (v < 0 || v >= limit)
+      return fail(BSG_ERR_BOUNDS, "Tested subscript out of bounds (%s%d not in 1..%d).", label, (int)(v + 1), limit);
+    out[i] = (int)v;
+  }
+  if (maxmult) *maxmult = ind ? max_mult(out, limit) : 1;
+  return BSG_OK;
+}
+
 int upload_index(bsg_bed *h, const int *ind, int len, int limit, DevBuf &buf, const int **dev) {
   *dev = nullptr;
   if (!ind) return BSG_OK;
-  std::vector<int> z((size_t)(len > 0 ? len : 1));
-  for (int i = 0; i < len; i++) {
-    long long v = (long long)ind[i] - 1;
-    if (v < 0 || v >= limit) return fail(BSG_ERR_BOUNDS, "Tested subscript out of bounds (%d not in 1..%d).", ind[i], limit);
-    z[i] = (int)v;
-  }
+  std::vector<int> z;
+  BSG_TRY(host_index(ind, len, limit, "", z));
   BSG_TRY(buf.ensure((size_t)(len > 0 ? len : 1) * sizeof(int)));
-  BSG_CUDA(cudaMemcpyAsync(buf.p, z.data(), (size_t)len * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+  if (len > 0) BSG_CUDA(cudaMemcpyAsync(buf.p, z.data(), (size_t)len * sizeof(int), cudaMemcpyHostToDevice, h->stream));
   BSG_CUDA(cudaStreamSynchronize(h->stream));  // z goes out of scope
   *dev = buf.as<int>();
   return BSG_OK;
+}
+
+int genotypes_check(const bsg_bed *h, const char *who) {
+  if (h->fbm_generic && !h->dos_scale)
+    return fail(BSG_ERR_TYPE, "%s hard calls or dosages (codes multiples of 1 / D); this FBM.code256 holds other values.", who);
+  return BSG_OK;
+}
+
+int genotypes(bsg_bed *h, Bufs &b, Genotypes *g) {
+  *g = Genotypes{};
+  g->raw = h->raw;
+  if (!h->fbm_generic) {
+    g->P = h->A;
+    g->stride = h->strideA;
+    return BSG_OK;
+  }
+  BSG_TRY(dosage_build(h));
+  g->P = h->dosV;
+  g->stride = h->dosStride;
+  g->D = h->dos_scale;
+  g->lut = dosage_lut(h, b);
+  g->dosage = true;
+  return BSG_OK;
+}
+
+int *dosage_lut(const bsg_bed *h, Bufs &b) {
+  std::vector<int> lut(256);
+  for (int c = 0; c < 256; c++)
+    lut[c] = h->code256[c] != h->code256[c] ? -1 : (int)nearbyint(h->dos_scale * h->code256[c]);
+  int *d_lut = nullptr;
+  b.up(&d_lut, lut, h->stream);
+  return d_lut;
 }
 
 }  // namespace bsg

@@ -345,14 +345,6 @@ __global__ void k_gwas_stats(const long long *__restrict__ xs, const double *__r
 
 static thread_local double g_last_ms = 0;
 
-struct Events {
-  cudaEvent_t ev[2] = {nullptr, nullptr};
-  ~Events() {
-    for (auto e : ev)
-      if (e) cudaEventDestroy(e);
-  }
-};
-
 // e = bits - exponent(max |v|) - hb (pick_e), hb as hb_bits of the matvecs
 static int host_pick_e(double m, int hb, int bits) {
   int ex = 0;
@@ -361,11 +353,6 @@ static int host_pick_e(double m, int hb, int bits) {
     return bits - ex - hb;
   }
   return 0;
-}
-static int hb_bits(int maxmult) {
-  int b = 0;
-  while ((1 << b) < maxmult) b++;
-  return b >= 8 ? b + 1 : b;
 }
 
 template <int NT>
@@ -388,9 +375,7 @@ int bsg_univlinreg(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, i
   using namespace gwas;
   if (!h) return fail(BSG_ERR_ARG, "null handle");
   const bool dos = h->fbm_generic != 0;
-  if (dos && !h->dos_scale)
-    return fail(BSG_ERR_TYPE, "big_univLinReg on the device needs hard calls or dosages (codes multiples of 1 / D); this "
-                              "FBM.code256 holds other values.");
+  BSG_TRY(genotypes_check(h, "big_univLinReg on the device needs"));
   BSG_TRY(bind_device(h));
   if (!ind_row) nr = h->n;
   if (!ind_col) nc = h->m;
@@ -398,20 +383,10 @@ int bsg_univlinreg(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, i
   if (nr - K - 1 < 1) return fail(BSG_ERR_ARG, "Not enough rows of ind.train for %d covariate vectors.", K);
   if (!U || !y || (nc > 0 && (!estim || !std_err))) return fail(BSG_ERR_ARG, "null argument");
   const int n = h->n;
-  std::vector<int> row0(nr), mult(n, 0);
+  std::vector<int> row0, col0;
   int maxmult = 1;
-  for (int r = 0; r < nr; r++) {
-    const int i = ind_row ? ind_row[r] : r + 1;
-    if (i < 1 || i > n) return fail(BSG_ERR_BOUNDS, "Tested subscript out of bounds (%d not in 1..%d).", i, n);
-    row0[r] = i - 1;
-    maxmult = std::max(maxmult, ++mult[i - 1]);
-  }
-  std::vector<int> col0(std::max(nc, 1));
-  for (int c = 0; c < nc; c++) {
-    const int j = ind_col ? ind_col[c] : c + 1;
-    if (j < 1 || j > h->m) return fail(BSG_ERR_BOUNDS, "Tested subscript out of bounds (%d not in 1..%d).", j, h->m);
-    col0[c] = j - 1;
-  }
+  BSG_TRY(host_index(ind_row, nr, n, "", row0, &maxmult));
+  BSG_TRY(host_index(ind_col, nc, h->m, "", col0));
   for (int r = 0; r < nr; r++)
     if (!std::isfinite(y[r])) return fail(BSG_ERR_ARG, "'y.train' must be finite (entry %d is not).", r + 1);
   for (int64_t t = 0; t < (int64_t)nr * K; t++)
@@ -443,7 +418,6 @@ int bsg_univlinreg(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, i
   if (!(fabs(uu1 - nr) <= 1e-6 * nr))
     return fail(BSG_ERR_ARG, "U must have orthonormal columns spanning the intercept (|U'1|^2 = %g, n = %d).", uu1, nr);
   const double yres = yy - uyy, df = (double)(nr - K - 1);
-  const double D = dos ? (double)h->dos_scale : 1.0;
 
   // vectors: 0 = y_c (60 bits, 8 digits), 1 + k = u_k (30 bits, 4 digits); passes of at most SMAX slices
   const int V = K + 1, hb = hb_bits(maxmult);
@@ -479,41 +453,35 @@ int bsg_univlinreg(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, i
                                "%.0f are free.", (double)need, nc, n, V, (double)fr);
   g_last_ms = 0;
   if (nc == 0) return BSG_OK;
-  if (dos) BSG_TRY(dosage_build(h));
 
   cudaStream_t s = h->stream;
   Bufs b;
+  Genotypes g;
+  BSG_TRY(genotypes(h, b, &g));
+  const double D = g.dosage ? g.D : 1.0;
   long long *d_Q, *d_part, *d_xs;
   uint8_t *d_dig;
   double *d_S, *d_u1, *d_uy, *d_est, *d_se;
-  int *d_cols, *d_mult = nullptr, *d_lut = nullptr;
-  cudaError_t err = b.alloc(&d_Q, (size_t)maxvp * n);
-  if (err == cudaSuccess) err = b.alloc(&d_dig, dig_bytes);
-  if (err == cudaSuccess) err = b.alloc(&d_part, (size_t)nlines_pad * SMAX);
-  if (err == cudaSuccess) err = b.alloc(&d_xs, (size_t)3 * nc);
-  if (err == cudaSuccess) err = b.alloc(&d_S, (size_t)V * nc);
-  if (err == cudaSuccess) err = b.alloc(&d_est, (size_t)nc);
-  if (err == cudaSuccess) err = b.alloc(&d_se, (size_t)nc);
-  if (err == cudaSuccess) err = b.up(&d_u1, u1, s);
-  if (err == cudaSuccess) err = b.up(&d_uy, uy, s);
-  if (err == cudaSuccess) err = b.up(&d_cols, col0.data(), (size_t)nc, s);
-  if (err == cudaSuccess && dos) err = b.up(&d_mult, mult, s);
-  std::vector<int> lut(256);
-  if (dos) {
-    for (int c = 0; c < 256; c++)
-      lut[c] = h->code256[c] != h->code256[c] ? -1 : (int)nearbyint(h->dos_scale * h->code256[c]);
-    if (err == cudaSuccess) err = b.up(&d_lut, lut, s);
+  int *d_cols, *d_mult = nullptr;
+  b.alloc(&d_Q, (size_t)maxvp * n);
+  b.alloc(&d_dig, dig_bytes);
+  b.alloc(&d_part, (size_t)nlines_pad * SMAX);
+  b.alloc(&d_xs, (size_t)3 * nc);
+  b.alloc(&d_S, (size_t)V * nc);
+  b.alloc(&d_est, (size_t)nc);
+  b.alloc(&d_se, (size_t)nc);
+  b.up(&d_u1, u1, s);
+  b.up(&d_uy, uy, s);
+  b.up(&d_cols, col0.data(), (size_t)nc, s);
+  if (g.dosage) {  // how many times ind.train holds each sample
+    std::vector<int> mult(n, 0);
+    for (int i : row0) mult[i]++;
+    b.up(&d_mult, mult, s);
   }
-  if (err != cudaSuccess) {
-    cudaGetLastError();
-    return fail(err == cudaErrorMemoryAllocation ? BSG_ERR_ALLOC : BSG_ERR_CUDA, "big_univLinReg scratch (%s)",
-                cudaGetErrorString(err));
-  }
-  Events tm;
-  BSG_CUDA(cudaEventCreate(&tm.ev[0]));
-  BSG_CUDA(cudaEventCreate(&tm.ev[1]));
+  BSG_TRY(b.status("big_univLinReg scratch"));
+  CallTimer tm;
   BSG_CUDA(cudaStreamSynchronize(s));
-  if (!dos) {  // sum x, sum x^2, NA count from the column counts over ind.train (multiplicities included)
+  if (!g.dosage) {  // sum x, sum x^2, NA count from the column counts over ind.train (multiplicities included)
     int32_t *d_cnt = nullptr;
     BSG_TRY(col_counts_dev(h, ind_row, nr, ind_col, nc, &d_cnt));
     k_gwas_xs_counts<<<(nc + 255) / 256, 256, 0, s>>>(d_cnt, nc, d_xs);
@@ -526,7 +494,7 @@ int bsg_univlinreg(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, i
     long long *Q = Qh.data() + (size_t)v * n;
     for (int r = 0; r < nr; r++) Q[row0[r]] += llrint(ldexp(x[r], ebits[v]));
   }
-  BSG_CUDA(cudaEventRecord(tm.ev[0], s));
+  BSG_CUDA(tm.start(s));
   int nsm = 132;
   cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, h->device);
   for (size_t p = 0; p < passes.size(); p++) {
@@ -543,18 +511,18 @@ int bsg_univlinreg(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, i
     BSG_CUDA(cudaMemcpyAsync(d_Q, Qh.data() + (size_t)pv[0] * n, pv.size() * n * sizeof(long long),
                              cudaMemcpyHostToDevice, s));
     BSG_CUDA(cudaMemsetAsync(d_part, 0, (size_t)nlines_pad * SMAX * sizeof(long long), s));
-    if (dos) {
+    if (g.dosage) {
       int8_t *dg = reinterpret_cast<int8_t *>(d_dig);
       k_gwas_digits_rows<<<(int)std::min<int64_t>(((int64_t)S * n + 255) / 256, 4096), 256, 0, s>>>(d_Q, n, S, map, dg);
-      k_gwas_dos<<<nc, DT, 0, s>>>(h->raw, n, d_lut, d_cols, d_mult, dg, S, d_part, p == 0 ? d_xs : nullptr);
+      k_gwas_dos<<<nc, DT, 0, s>>>(g.raw, n, g.lut, d_cols, d_mult, dg, S, d_part, p == 0 ? d_xs : nullptr);
       count_launch(2);
     } else {
       const int NT = (S + 7) / 8;
       const int64_t units = (int64_t)nchunks * 8 * NT * 32;
       k_gwas_digits<<<(int)std::min<int64_t>((units + 255) / 256, 8192), 256, 0, s>>>(d_Q, n, nchunks, NT, map, d_dig);
       GArgs a;
-      a.P = h->A;
-      a.stride = h->strideA;
+      a.P = g.P;
+      a.stride = g.stride;
       a.lines = d_cols;
       a.nlines = nc;
       a.nlines_pad = nlines_pad;
@@ -593,13 +561,11 @@ int bsg_univlinreg(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, i
   k_gwas_stats<<<(nc + 255) / 256, 256, 0, s>>>(d_xs, d_S, nc, K, d_u1, d_uy, (long long)nr, D, df, yres, d_est, d_se);
   count_launch();
   BSG_CUDA(cudaGetLastError());
-  BSG_CUDA(cudaEventRecord(tm.ev[1], s));
+  BSG_CUDA(tm.stop(s));
   BSG_CUDA(cudaMemcpyAsync(estim, d_est, (size_t)nc * sizeof(double), cudaMemcpyDeviceToHost, s));
   BSG_CUDA(cudaMemcpyAsync(std_err, d_se, (size_t)nc * sizeof(double), cudaMemcpyDeviceToHost, s));
   BSG_CUDA(cudaStreamSynchronize(s));
-  float ms = 0;
-  cudaEventElapsedTime(&ms, tm.ev[0], tm.ev[1]);
-  g_last_ms = ms;
+  g_last_ms = tm.ms();
   return BSG_OK;
 }
 

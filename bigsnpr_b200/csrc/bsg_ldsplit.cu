@@ -378,20 +378,17 @@ static int run_layers(Run &R, int device, cudaStream_t st, const long long *src_
   float *d_E = nullptr;
   int *d_elen = nullptr;
   double *d_pos = nullptr;
-  cudaError_t e = R.b.up(&d_eoff, eoff, st);
-  if (e == cudaSuccess) e = R.b.alloc(&d_E, (size_t)eoff[m]);
-  if (e == cudaSuccess) e = R.b.alloc(&d_elen, (size_t)m);
-  if (e == cudaSuccess) e = R.b.up(&d_pos, pos, (size_t)m, st);
-  if (e == cudaSuccess) e = R.b.alloc(&R.C1, ns * mK);
-  if (e == cudaSuccess) e = R.b.alloc(&R.best, ns * mK);
-  if (e == cudaSuccess) e = R.b.alloc(&R.C2, (size_t)ns * 2 * m);
-  if (e == cudaSuccess) e = R.b.up(&R.Sv, U, st);
-  if (e == cudaSuccess) e = R.b.alloc(&R.active, (size_t)ns);
-  if (e == cudaSuccess) e = R.b.alloc(&R.layers, (size_t)ns);
-  if (e != cudaSuccess) {
-    cudaGetLastError();
-    return fail(e == cudaErrorMemoryAllocation ? BSG_ERR_ALLOC : BSG_ERR_CUDA, "snp_ldsplit state (%s)", cudaGetErrorString(e));
-  }
+  R.b.up(&d_eoff, eoff, st);
+  R.b.alloc(&d_E, (size_t)eoff[m]);
+  R.b.alloc(&d_elen, (size_t)m);
+  R.b.up(&d_pos, pos, (size_t)m, st);
+  R.b.alloc(&R.C1, ns * mK);
+  R.b.alloc(&R.best, ns * mK);
+  R.b.alloc(&R.C2, (size_t)ns * 2 * m);
+  R.b.up(&R.Sv, U, st);
+  R.b.alloc(&R.active, (size_t)ns);
+  R.b.alloc(&R.layers, (size_t)ns);
+  BSG_TRY(R.b.status("snp_ldsplit state"));
   Timer tm;
   BSG_CUDA(cudaEventRecord(tm.ev[0], st));
   k_build_E<FROM_CSC><<<grid_for((long long)m * 32, 256), 256, 0, st>>>(src_p, src_rows, src_vals, m, d_pos, min_size, smax,
@@ -481,10 +478,8 @@ int bsg_ldcorr_open(int m, const long long *p, const int *i, const double *x, in
   if (e == cudaSuccess) e = cudaMalloc(&c->i, nnz * sizeof(int));
   if (e == cudaSuccess) e = cudaMalloc(&c->x, nnz * sizeof(double));
   if (e != cudaSuccess) {
-    cudaGetLastError();
     bsg_ldcorr_close(c);
-    return fail(e == cudaErrorMemoryAllocation ? BSG_ERR_ALLOC : BSG_ERR_CUDA, "corr does not fit in device memory (%s)",
-                cudaGetErrorString(e));
+    return alloc_fail(e, "corr does not fit in device memory");
   }
   e = cudaMemcpy(c->p, p, (m + 1) * sizeof(long long), cudaMemcpyHostToDevice);
   if (e == cudaSuccess) e = cudaMemcpy(c->i, i, nnz * sizeof(int), cudaMemcpyHostToDevice);
@@ -532,14 +527,11 @@ int bsg_ldcorr_l_triplets(bsg_ldcorr *c, double thr_r2, double max_r2, long long
   long long *d_off = nullptr;
   int *d_li = nullptr, *d_lj = nullptr;
   double *d_lx = nullptr;
-  cudaError_t e = b.up(&d_off, off, st);
-  if (e == cudaSuccess) e = b.alloc(&d_li, n);
-  if (e == cudaSuccess) e = b.alloc(&d_lj, n);
-  if (e == cudaSuccess) e = b.alloc(&d_lx, n);
-  if (e != cudaSuccess) {
-    cudaGetLastError();
-    return fail(e == cudaErrorMemoryAllocation ? BSG_ERR_ALLOC : BSG_ERR_CUDA, "get_L triplets (%s)", cudaGetErrorString(e));
-  }
+  b.up(&d_off, off, st);
+  b.alloc(&d_li, n);
+  b.alloc(&d_lj, n);
+  b.alloc(&d_lx, n);
+  BSG_TRY(b.status("get_L triplets"));
   k_get_L<<<grid_for((long long)c->m * 32, 256), 256, 0, st>>>(c->p, c->i, d_suf, d_rs, d_off, c->m, d_li, d_lj, d_lx);
   count_launch();
   BSG_CUDA(cudaGetLastError());
@@ -580,16 +572,13 @@ int bsg_ldsplit(bsg_ldcorr *c, double thr_r2, int min_size, const int *max_size,
                             nrow * (sizeof(int) + 3 * sizeof(double)) + n_max_size * T * sizeof(int)));
   int *d_uniq = nullptr, *d_kept = nullptr, *d_path = nullptr;
   double *d_cost = nullptr, *d_cost2 = nullptr, *d_perc = nullptr;
-  cudaError_t e = b.up(&d_uniq, uniq, st);
-  if (e == cudaSuccess) e = b.alloc(&d_kept, nrow);
-  if (e == cudaSuccess) e = b.alloc(&d_cost, nrow);
-  if (e == cudaSuccess) e = b.alloc(&d_cost2, nrow);
-  if (e == cudaSuccess) e = b.alloc(&d_perc, nrow);
-  if (e == cudaSuccess) e = b.alloc(&d_path, n_max_size * T);
-  if (e != cudaSuccess) {
-    cudaGetLastError();
-    return fail(e == cudaErrorMemoryAllocation ? BSG_ERR_ALLOC : BSG_ERR_CUDA, "snp_ldsplit results (%s)", cudaGetErrorString(e));
-  }
+  b.up(&d_uniq, uniq, st);
+  b.alloc(&d_kept, nrow);
+  b.alloc(&d_cost, nrow);
+  b.alloc(&d_cost2, nrow);
+  b.alloc(&d_perc, nrow);
+  b.alloc(&d_path, n_max_size * T);
+  BSG_TRY(b.status("snp_ldsplit results"));
   Timer tm;
   BSG_CUDA(cudaEventRecord(tm.ev[0], st));
   BSG_CUDA(cudaMemsetAsync(d_path, 0, n_max_size * T * sizeof(int), st));
@@ -655,14 +644,10 @@ int bsg_ldsplit_costs(int m, const long long *lp, const int *li, const double *l
     long long *d_lp = nullptr;
     int *d_li = nullptr;
     double *d_lx = nullptr;
-    cudaError_t e = b.up(&d_lp, lp, (size_t)m + 2, st);
-    if (e == cudaSuccess) e = b.up(&d_li, li, (size_t)nl, st);
-    if (e == cudaSuccess) e = b.up(&d_lx, lx, (size_t)nl, st);
-    if (e != cudaSuccess) {
-      cudaGetLastError();
-      return fail(e == cudaErrorMemoryAllocation ? BSG_ERR_ALLOC : BSG_ERR_CUDA, "L does not fit in device memory (%s)",
-                  cudaGetErrorString(e));
-    }
+    b.up(&d_lp, lp, (size_t)m + 2, st);
+    b.up(&d_li, li, (size_t)nl, st);
+    b.up(&d_lx, lx, (size_t)nl, st);
+    BSG_TRY(b.status("L does not fit in device memory"));
     Run R;
     rc = run_layers<true>(R, device, st, d_lp, d_li, d_lx, m, pos_scaled, min_size, std::vector<int>{max_size}, max_K,
                           max_cost, 0);

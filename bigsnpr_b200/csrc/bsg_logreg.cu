@@ -303,14 +303,6 @@ __global__ void k_logreg_check_counts(const int32_t *__restrict__ cnt, int nc, i
 
 static thread_local double g_last_ms = 0;
 
-struct Events {
-  cudaEvent_t ev[2] = {nullptr, nullptr};
-  ~Events() {
-    for (auto e : ev)
-      if (e) cudaEventDestroy(e);
-  }
-};
-
 // entries in Idx order, each group padded to TE with (K, K) fillers; tile g per TE entries
 static void entries(int K, std::vector<short2> &ent, std::vector<uint8_t> &tg) {
   const Idx ix(K);
@@ -359,10 +351,7 @@ int bsg_univlogreg(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, i
                    int *niter) {
   using namespace logreg;
   if (!h) return fail(BSG_ERR_ARG, "null handle");
-  const bool dos = h->fbm_generic != 0;
-  if (dos && !h->dos_scale)
-    return fail(BSG_ERR_TYPE, "big_univLogReg on the device needs hard calls or dosages (codes multiples of 1 / D); this "
-                              "FBM.code256 holds other values.");
+  BSG_TRY(genotypes_check(h, "big_univLogReg on the device needs"));
   BSG_TRY(bind_device(h));
   if (!ind_row) nr = h->n;
   if (!ind_col) nc = h->m;
@@ -371,18 +360,9 @@ int bsg_univlogreg(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, i
   if (maxiter < 1) return fail(BSG_ERR_ARG, "'maxiter' must be at least 1.");
   if (!U || !gamma0 || !y01 || (nc > 0 && (!estim || !std_err || !niter))) return fail(BSG_ERR_ARG, "null argument");
   const int n = h->n;
-  std::vector<int> row0(nr);
-  for (int r = 0; r < nr; r++) {
-    const int i = ind_row ? ind_row[r] : r + 1;
-    if (i < 1 || i > n) return fail(BSG_ERR_BOUNDS, "Tested subscript out of bounds (%d not in 1..%d).", i, n);
-    row0[r] = i - 1;
-  }
-  std::vector<int> col0(std::max(nc, 1));
-  for (int c = 0; c < nc; c++) {
-    const int j = ind_col ? ind_col[c] : c + 1;
-    if (j < 1 || j > h->m) return fail(BSG_ERR_BOUNDS, "Tested subscript out of bounds (%d not in 1..%d).", j, h->m);
-    col0[c] = j - 1;
-  }
+  std::vector<int> row0, col0;
+  BSG_TRY(host_index(ind_row, nr, n, "", row0));
+  BSG_TRY(host_index(ind_col, nc, h->m, "", col0));
   for (int r = 0; r < nr; r++)
     if (!(y01[r] == 0.0 || y01[r] == 1.0)) return fail(BSG_ERR_ARG, "'y01.train' must be 0 or 1 (entry %d is not).", r + 1);
   for (int64_t t = 0; t < (int64_t)nr * K; t++)
@@ -403,51 +383,40 @@ int bsg_univlogreg(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, i
                                "%.0f are free.", (double)need, nc, nr, K, (double)fr);
   g_last_ms = 0;
   if (nc == 0) return BSG_OK;
-  if (dos) BSG_TRY(dosage_build(h));
 
   cudaStream_t s = h->stream;
+  Bufs b;
+  Genotypes g;
+  BSG_TRY(genotypes(h, b, &g));
   std::vector<double> Ur((size_t)nr * K);  // row-major [nr][K]
   for (int k = 0; k < K; k++)
     for (int r = 0; r < nr; r++) Ur[(size_t)r * K + k] = U[(size_t)k * nr + r];
   std::vector<short2> ent;
   std::vector<uint8_t> tg;
   entries(K, ent, tg);
-  Bufs b;
   double *d_U, *d_y, *d_g0, *d_est, *d_se;
-  int *d_rows, *d_cols, *d_it, *d_queue, *d_lut = nullptr;
+  int *d_rows, *d_cols, *d_it, *d_queue;
   uint8_t *d_bad, *d_tg;
   short2 *d_ent;
-  cudaError_t err = b.up(&d_U, Ur, s);
-  if (err == cudaSuccess) err = b.up(&d_y, y01, (size_t)nr, s);
-  if (err == cudaSuccess) err = b.up(&d_g0, gamma0, (size_t)K, s);
-  if (err == cudaSuccess) err = b.up(&d_rows, row0, s);
-  if (err == cudaSuccess) err = b.up(&d_cols, col0.data(), (size_t)nc, s);
-  if (err == cudaSuccess) err = b.up(&d_ent, ent, s);
-  if (err == cudaSuccess) err = b.up(&d_tg, tg, s);
-  if (err == cudaSuccess) err = b.alloc(&d_bad, (size_t)nc);
-  if (err == cudaSuccess) err = b.alloc(&d_est, (size_t)nc);
-  if (err == cudaSuccess) err = b.alloc(&d_se, (size_t)nc);
-  if (err == cudaSuccess) err = b.alloc(&d_it, (size_t)nc);
-  if (err == cudaSuccess) err = b.alloc(&d_queue, 1);
-  if (dos) {
-    std::vector<int> lut(256);
-    for (int c = 0; c < 256; c++)
-      lut[c] = h->code256[c] != h->code256[c] ? -1 : (int)nearbyint(h->dos_scale * h->code256[c]);
-    if (err == cudaSuccess) err = b.up(&d_lut, lut, s);
-  }
-  if (err != cudaSuccess) {
-    cudaGetLastError();
-    return fail(err == cudaErrorMemoryAllocation ? BSG_ERR_ALLOC : BSG_ERR_CUDA, "big_univLogReg scratch (%s)",
-                cudaGetErrorString(err));
-  }
+  b.up(&d_U, Ur, s);
+  b.up(&d_y, y01, (size_t)nr, s);
+  b.up(&d_g0, gamma0, (size_t)K, s);
+  b.up(&d_rows, row0, s);
+  b.up(&d_cols, col0.data(), (size_t)nc, s);
+  b.up(&d_ent, ent, s);
+  b.up(&d_tg, tg, s);
+  b.alloc(&d_bad, (size_t)nc);
+  b.alloc(&d_est, (size_t)nc);
+  b.alloc(&d_se, (size_t)nc);
+  b.alloc(&d_it, (size_t)nc);
+  b.alloc(&d_queue, 1);
+  BSG_TRY(b.status("big_univLogReg scratch"));
   BSG_CUDA(cudaMemsetAsync(d_queue, 0, sizeof(int), s));
-  Events tm;
-  BSG_CUDA(cudaEventCreate(&tm.ev[0]));
-  BSG_CUDA(cudaEventCreate(&tm.ev[1]));
+  CallTimer tm;
   BSG_CUDA(cudaStreamSynchronize(s));
-  BSG_CUDA(cudaEventRecord(tm.ev[0], s));
-  if (dos) {
-    k_logreg_check_dos<<<nc, 256, 0, s>>>(h->raw, n, d_lut, d_cols, d_rows, nr, d_bad);
+  BSG_CUDA(tm.start(s));
+  if (g.dosage) {
+    k_logreg_check_dos<<<nc, 256, 0, s>>>(g.raw, n, g.lut, d_cols, d_rows, nr, d_bad);
     count_launch();
   } else {
     int32_t *d_cnt = nullptr;
@@ -456,9 +425,9 @@ int bsg_univlogreg(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, i
     count_launch();
   }
   LArgs a;
-  a.P = dos ? h->dosV : h->A;
-  a.stride = dos ? h->dosStride : h->strideA;
-  a.D = dos ? (double)h->dos_scale : 0.0;
+  a.P = g.P;
+  a.stride = g.stride;
+  a.D = g.D;
   a.rows = d_rows;
   a.U = d_U;
   a.y = d_y;
@@ -479,14 +448,12 @@ int bsg_univlogreg(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, i
   k_logreg<<<grid, LT, lay.bytes, s>>>(a);
   count_launch();
   BSG_CUDA(cudaGetLastError());
-  BSG_CUDA(cudaEventRecord(tm.ev[1], s));
+  BSG_CUDA(tm.stop(s));
   BSG_CUDA(cudaMemcpyAsync(estim, d_est, (size_t)nc * sizeof(double), cudaMemcpyDeviceToHost, s));
   BSG_CUDA(cudaMemcpyAsync(std_err, d_se, (size_t)nc * sizeof(double), cudaMemcpyDeviceToHost, s));
   BSG_CUDA(cudaMemcpyAsync(niter, d_it, (size_t)nc * sizeof(int), cudaMemcpyDeviceToHost, s));
   BSG_CUDA(cudaStreamSynchronize(s));
-  float ms = 0;
-  cudaEventElapsedTime(&ms, tm.ev[0], tm.ev[1]);
-  g_last_ms = ms;
+  g_last_ms = tm.ms();
   return BSG_OK;
 }
 

@@ -559,16 +559,6 @@ static int launch_cap(int64_t work, int block, int cap) {
 
 static int launch_cap_pub_impl(int64_t work) { return launch_cap(work, 256, 132 * 16); }
 
-// Head-room bits for sums of up to `maxmult` quantised values: with e = 60 - ex - hb every |v 2^e| < 2^(60 - hb), and
-// while 60 - hb >= 53 that double is already an integer, so |rint(v 2^e)| < 2^(60 - hb) and the sum stays below 2^60.
-// From hb = 8 on, rint may round an entry just below the binade up to 2^(60 - hb) itself and 2^hb of them reach 2^60:
-// one more bit there keeps every sum below 2^60 (k_corr adds 8 of them in int64).
-static int hb_bits(int maxmult) {
-  int b = 0;
-  while ((1 << b) < maxmult) b++;
-  return b >= 8 ? b + 1 : b;
-}
-
 // Digits of the k_pmv layout for a vector over the selected columns (dir 0: lines = samples of copy B) or over the
 // selected samples (dir 1: lines = SNP columns of copy A).  nv = 1: one vector of make_vals(mode, x, p1, p2), 60 bits,
 // its second value into s_dig2 when `two`.  nv = 2: the vectors x and xb (mode 0, 30 bits each, 4 + 4 slices of s_dig1;
@@ -1284,17 +1274,6 @@ static bool is_identity(const int *ind, int len, int limit) {
   return true;
 }
 
-static int max_mult(std::vector<int> z) {
-  if (z.empty()) return 1;
-  std::sort(z.begin(), z.end());
-  int best = 1, run = 1;
-  for (size_t i = 1; i < z.size(); i++) {
-    run = (z[i] == z[i - 1]) ? run + 1 : 1;
-    best = std::max(best, run);
-  }
-  return best;
-}
-
 }  // namespace bsg
 
 using namespace bsg;
@@ -1331,14 +1310,8 @@ int bsg_view_create(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, 
   int rc = BSG_OK;
   std::vector<int> zr, zc, uniq, gat;
   if (!v->row_identity) {
-    zr.resize(nr);
-    for (int i = 0; i < nr && !rc; i++) {
-      long long t = (long long)ind_row[i] - 1;
-      if (t < 0 || t >= h->n) rc = fail(BSG_ERR_BOUNDS, "Tested subscript out of bounds (row %d not in 1..%d).", ind_row[i], h->n);
-      zr[i] = (int)t;
-    }
+    rc = host_index(ind_row, nr, h->n, "row ", zr, &v->row_maxmult);
     if (!rc) {
-      v->row_maxmult = max_mult(zr);
       uniq = zr;
       std::sort(uniq.begin(), uniq.end());
       uniq.erase(std::unique(uniq.begin(), uniq.end()), uniq.end());
@@ -1353,16 +1326,8 @@ int bsg_view_create(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, 
     v->nru = h->n;
   }
   if (!rc && !v->col_identity) {
-    zc.resize(nc);
-    for (int j = 0; j < nc && !rc; j++) {
-      long long t = (long long)ind_col[j] - 1;
-      if (t < 0 || t >= h->m) rc = fail(BSG_ERR_BOUNDS, "Tested subscript out of bounds (column %d not in 1..%d).", ind_col[j], h->m);
-      zc[j] = (int)t;
-    }
-    if (!rc) {
-      v->col_maxmult = max_mult(zc);
-      rc = dev_copy((void **)&v->d_col, zc.data(), (size_t)nc * sizeof(int), s);
-    }
+    rc = host_index(ind_col, nc, h->m, "column ", zc, &v->col_maxmult);
+    if (!rc) rc = dev_copy((void **)&v->d_col, zc.data(), (size_t)nc * sizeof(int), s);
   }
   if (!rc && v->has_scaling) {
     rc = dev_copy((void **)&v->d_center, center, (size_t)nc * sizeof(double), s);

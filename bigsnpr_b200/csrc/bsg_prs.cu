@@ -372,14 +372,6 @@ __global__ void __launch_bounds__(DOS_T) k_prs_dos(const DArgs a) {
 
 static thread_local double g_last_ms = 0;  // of the last call on this thread
 
-struct Events {
-  cudaEvent_t ev[2] = {nullptr, nullptr};
-  ~Events() {
-    for (auto e : ev)
-      if (e) cudaEventDestroy(e);
-  }
-};
-
 }  // namespace prs
 }  // namespace bsg
 
@@ -394,18 +386,12 @@ int bsg_prs_grid(bsg_bed *h, const int *ind_row, int nr, int nsets, const int *s
   if (!h || nsets < 0 || nthr < 1 || (nsets > 0 && !set_len) || (!thr && nthr != 1) || (thr && !lpS))
     return fail(BSG_ERR_ARG, "null argument or bad lengths");
   const bool dos = h->fbm_generic != 0;
-  if (dos && !h->dos_scale)
-    return fail(BSG_ERR_TYPE, "snp_PRS on the device needs hard calls or dosages (codes multiples of 1 / D); this "
-                              "FBM.code256 holds other values.");
+  BSG_TRY(genotypes_check(h, "snp_PRS on the device needs"));
   BSG_TRY(bind_device(h));
   if (!ind_row) nr = h->n;
   if (nr < 0) return fail(BSG_ERR_ARG, "bad length of ind.row");
-  std::vector<int> row0(std::max(nr, 1));
-  for (int r = 0; r < nr; r++) {
-    const int i = ind_row ? ind_row[r] : r + 1;
-    if (i < 1 || i > h->n) return fail(BSG_ERR_BOUNDS, "ind.row out of range");
-    row0[r] = i - 1;
-  }
+  std::vector<int> row0;
+  BSG_TRY(host_index(ind_row, nr, h->n, "", row0));
   // thresholds in stable decreasing order (R's order(thr.list, decreasing = TRUE))
   std::vector<int> ord(nthr);
   std::iota(ord.begin(), ord.end(), 0);
@@ -483,48 +469,31 @@ int bsg_prs_grid(bsg_bed *h, const int *ind_row, int nr, int nsets, const int *s
 
   cudaStream_t s = h->stream;
   Bufs b;
+  int *d_lut = dos ? dosage_lut(h, b) : nullptr;
   int *d_lines, *d_goff, *d_send, *d_col, *d_slot, *d_row;
   uint8_t *d_kind, *d_dig;
   double *d_v, *d_cst, *d_S;
   long long *d_kc, *d_base = nullptr;
   Scal *d_sc;
   void *d_out;
-  cudaError_t err = b.up(&d_lines, lines, s);
-  if (err == cudaSuccess) err = b.up(&d_goff, grp_off, s);
-  if (err == cudaSuccess) err = b.up(&d_send, step_end, s);
-  if (err == cudaSuccess) err = b.up(&d_col, col_of, s);
-  if (err == cudaSuccess) err = b.up(&d_slot, long_slot, s);
-  if (err == cudaSuccess) err = b.up(&d_row, row0.data(), (size_t)nr, s);
-  if (err == cudaSuccess) err = b.up(&d_kind, kind, s);
-  if (err == cudaSuccess) err = b.up(&d_v, v, s);
-  if (err == cudaSuccess) err = b.up(&d_cst, cst, s);
-  if (err == cudaSuccess) err = b.alloc(&d_dig, (size_t)std::max<int64_t>(ngrp, 1) * 256);
-  if (err == cudaSuccess) err = b.alloc(&d_kc, (size_t)ncol * 8);
-  if (err == cudaSuccess) err = b.alloc(&d_sc, (size_t)std::max(nsets, 1));
-  if (err == cudaSuccess && nlong) err = b.alloc(&d_base, (size_t)nlong * nblocks * 64 * 256);
-  if (err == cudaSuccess) err = b.alloc(&d_S, (size_t)ncol * n);
-  if (err == cudaSuccess) err = b.alloc((uint8_t **)&d_out, (size_t)ncol * nr * osz);
-  if (err != cudaSuccess) {
-    cudaGetLastError();
-    return fail(err == cudaErrorMemoryAllocation ? BSG_ERR_ALLOC : BSG_ERR_CUDA, "snp_grid_PRS scratch (%s)",
-                cudaGetErrorString(err));
-  }
-  int *d_lut = nullptr;
-  std::vector<int> lut(256);
-  if (dos) {
-    for (int c = 0; c < 256; c++)
-      lut[c] = h->code256[c] != h->code256[c] ? -1 : (int)nearbyint(h->dos_scale * h->code256[c]);
-    err = b.up(&d_lut, lut, s);
-    if (err != cudaSuccess) {
-      cudaGetLastError();
-      return fail(err == cudaErrorMemoryAllocation ? BSG_ERR_ALLOC : BSG_ERR_CUDA, "snp_grid_PRS scratch (%s)",
-                  cudaGetErrorString(err));
-    }
-  }
-  Events tm;
-  BSG_CUDA(cudaEventCreate(&tm.ev[0]));
-  BSG_CUDA(cudaEventCreate(&tm.ev[1]));
-  BSG_CUDA(cudaEventRecord(tm.ev[0], s));
+  b.up(&d_lines, lines, s);
+  b.up(&d_goff, grp_off, s);
+  b.up(&d_send, step_end, s);
+  b.up(&d_col, col_of, s);
+  b.up(&d_slot, long_slot, s);
+  b.up(&d_row, row0.data(), (size_t)nr, s);
+  b.up(&d_kind, kind, s);
+  b.up(&d_v, v, s);
+  b.up(&d_cst, cst, s);
+  b.alloc(&d_dig, (size_t)std::max<int64_t>(ngrp, 1) * 256);
+  b.alloc(&d_kc, (size_t)ncol * 8);
+  b.alloc(&d_sc, (size_t)std::max(nsets, 1));
+  if (nlong) b.alloc(&d_base, (size_t)nlong * nblocks * 64 * 256);
+  b.alloc(&d_S, (size_t)ncol * n);
+  b.alloc((uint8_t **)&d_out, (size_t)ncol * nr * osz);
+  BSG_TRY(b.status("snp_grid_PRS scratch"));
+  CallTimer tm;
+  BSG_CUDA(tm.start(s));
   BSG_CUDA(cudaMemsetAsync(d_sc, 0, (size_t)std::max(nsets, 1) * sizeof(Scal), s));
   for (int c = 0; c < nsets; c++) {
     const int64_t l0 = (int64_t)grp_off[c] * TL, len = (int64_t)(grp_off[c + 1] - grp_off[c]) * TL;
@@ -592,12 +561,10 @@ int bsg_prs_grid(bsg_bed *h, const int *ind_row, int nr, int nsets, const int *s
                                                                                         out_double, d_out);
   count_launch();
   BSG_CUDA(cudaGetLastError());
-  BSG_CUDA(cudaEventRecord(tm.ev[1], s));
+  BSG_CUDA(tm.stop(s));
   BSG_CUDA(cudaMemcpyAsync(out, d_out, (size_t)ncol * nr * osz, cudaMemcpyDeviceToHost, s));
   BSG_CUDA(cudaStreamSynchronize(s));
-  float ms = 0;
-  cudaEventElapsedTime(&ms, tm.ev[0], tm.ev[1]);
-  g_last_ms = ms;
+  g_last_ms = tm.ms();
   return BSG_OK;
 }
 

@@ -812,10 +812,8 @@ int bsg_sfbm_open(int nrow, int ncol, const double *p, const double *data, const
   if (e == cudaSuccess) e = cudaMalloc(&s->x, nv * sizeof(double));
   if (e == cudaSuccess) e = compact ? cudaMalloc(&s->first_i, (ncol ? ncol : 1) * sizeof(int)) : cudaMalloc(&s->rows, nv * sizeof(int));
   if (e != cudaSuccess) {
-    cudaGetLastError();
     bsg_sfbm_close(s);
-    return fail(e == cudaErrorMemoryAllocation ? BSG_ERR_ALLOC : BSG_ERR_CUDA, "SFBM does not fit in device memory (%s)",
-                cudaGetErrorString(e));
+    return alloc_fail(e, "SFBM does not fit in device memory");
   }
   e = cudaMemcpy(s->p, hp.data(), (ncol + 1) * sizeof(long long), cudaMemcpyHostToDevice);
   if (e == cudaSuccess && nnz) e = cudaMemcpy(s->x, vals.data(), (size_t)nnz * sizeof(double), cudaMemcpyHostToDevice);
@@ -890,14 +888,11 @@ int bsg_lassosum2(bsg_sfbm *corr, const double *beta_hat, int m, const int *ind_
   unsigned long long *d_ns = nullptr;
   BSG_CUDA(b.up(&d_sub, ind_sub, (size_t)m, st));
   BSG_CUDA(b.up(&d_bh, beta_hat, (size_t)m, st));
-  cudaError_t e = b.up(&d_lam, lambda, mg, st);
-  if (e == cudaSuccess) e = b.up(&d_dp1, delta_plus_one, mg, st);
-  if (e == cudaSuccess) e = b.alloc(&d_beta, mg);
-  if (e == cudaSuccess) e = b.alloc(&d_dot, (size_t)corr->ncol * ngrid);
-  if (e != cudaSuccess) {
-    cudaGetLastError();
-    return fail(e == cudaErrorMemoryAllocation ? BSG_ERR_ALLOC : BSG_ERR_CUDA, "lassosum2 state (%s)", cudaGetErrorString(e));
-  }
+  b.up(&d_lam, lambda, mg, st);
+  b.up(&d_dp1, delta_plus_one, mg, st);
+  b.alloc(&d_beta, mg);
+  b.alloc(&d_dot, (size_t)corr->ncol * ngrid);
+  BSG_TRY(b.status("lassosum2 state"));
   BSG_CUDA(b.alloc(&d_iter, (size_t)ngrid));
   BSG_CUDA(b.alloc(&d_ns, (size_t)ngrid));
   k_lassosum2<<<ngrid, LT, 0, st>>>(corr->p, corr->rows, corr->first_i, corr->x, corr->ncol, d_bh, m, d_sub, d_lam, d_dp1,
@@ -934,19 +929,18 @@ int bsg_sfbm_solve(bsg_sfbm *A, const double *b, const double *add_to_diag, int 
   double *d_b = nullptr, *d_d = nullptr, *d_x = nullptr, *d_r = nullptr, *d_p = nullptr, *d_t = nullptr;
   double *d_ppt = nullptr, *d_prr = nullptr;
   CgState *d_st = nullptr;
-  cudaError_t e = bf.up(&d_b, b, (size_t)n, st, A->device);
-  if (e == cudaSuccess) e = bf.up(&d_d, add_to_diag, (size_t)diag_len, st, A->device);
-  if (e == cudaSuccess) e = bf.alloc(&d_x, (size_t)n, A->device, st);
-  if (e == cudaSuccess) e = bf.alloc(&d_r, (size_t)n, A->device, st);
-  if (e == cudaSuccess) e = bf.alloc(&d_p, (size_t)n, A->device, st);
-  if (e == cudaSuccess) e = bf.alloc(&d_t, (size_t)n, A->device, st);
-  if (e == cudaSuccess) e = bf.alloc(&d_ppt, (size_t)nch, A->device, st);
-  if (e == cudaSuccess) e = bf.alloc(&d_prr, (size_t)nch, A->device, st);
-  if (e == cudaSuccess) e = bf.alloc(&d_st, 1, A->device, st);
-  if (e != cudaSuccess) {
-    cudaGetLastError();
+  bf.up(&d_b, b, (size_t)n, st, A->device);
+  bf.up(&d_d, add_to_diag, (size_t)diag_len, st, A->device);
+  bf.alloc(&d_x, (size_t)n, A->device, st);
+  bf.alloc(&d_r, (size_t)n, A->device, st);
+  bf.alloc(&d_p, (size_t)n, A->device, st);
+  bf.alloc(&d_t, (size_t)n, A->device, st);
+  bf.alloc(&d_ppt, (size_t)nch, A->device, st);
+  bf.alloc(&d_prr, (size_t)nch, A->device, st);
+  bf.alloc(&d_st, 1, A->device, st);
+  if (bf.err != cudaSuccess) {
     cudaStreamSynchronize(st);
-    return fail(e == cudaErrorMemoryAllocation ? BSG_ERR_ALLOC : BSG_ERR_CUDA, "solver state (%s)", cudaGetErrorString(e));
+    return bf.status("solver state");
   }
   k_cg_init<<<nch, CG_DT, 0, st>>>(d_b, n, d_x, d_r, d_p, d_prr);
   k_cg_init_fold<<<1, 32, 0, st>>>(d_prr, nch, d_st);
@@ -967,10 +961,8 @@ int bsg_sfbm_solve(bsg_sfbm *A, const double *b, const double *add_to_diag, int 
     int nsm = 132;
     cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, A->device);
     const int mgrid = (int)std::min<long long>(((long long)n * 32 + CG_MT - 1) / CG_MT, (long long)nsm * (2048 / CG_MT));
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-    BSG_CUDA(cudaEventCreate(&ev0));
-    e = cudaEventCreate(&ev1);
-    if (e == cudaSuccess) e = cudaEventRecord(ev0, st);
+    CallTimer tm;
+    cudaError_t e = tm.start(st);
     while (e == cudaSuccess && it < maxiter && !hs.done) {
       const int end = std::min(maxiter, it + CG_BLOCK);
       count_launch(4 * (end - it));
@@ -984,13 +976,10 @@ int bsg_sfbm_solve(bsg_sfbm *A, const double *b, const double *add_to_diag, int 
       if (e == cudaSuccess) e = cudaMemcpyAsync(&hs, d_st, sizeof hs, cudaMemcpyDeviceToHost, st);
       if (e == cudaSuccess) e = cudaStreamSynchronize(st);
     }
-    if (e == cudaSuccess) e = cudaEventRecord(ev1, st);
-    if (e == cudaSuccess) e = cudaEventSynchronize(ev1);
+    if (e == cudaSuccess) e = tm.stop(st);
     float ms = 0;
-    if (e == cudaSuccess) e = cudaEventElapsedTime(&ms, ev0, ev1);
+    if (e == cudaSuccess) e = tm.elapsed(&ms);
     A->last_solve_ms = ms;
-    cudaEventDestroy(ev0);
-    if (ev1) cudaEventDestroy(ev1);
     if (e != cudaSuccess) return cuda_fail(e, "conjugate gradient");
   }
   BSG_CUDA(cudaMemcpyAsync(x, d_x, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, st));
@@ -1051,27 +1040,22 @@ int bsg_ldpred2_auto_ex(bsg_sfbm *corr, const double *beta_hat, const double *n_
   double *d_bh = nullptr, *d_n = nullptr, *d_lv = nullptr, *d_pi = nullptr;
   int *d_sub = nullptr;
   uint32_t *d_rng = nullptr;
-  cudaError_t e = b.up(&d_bh, beta_hat, (size_t)m, st);
-  if (e == cudaSuccess) e = b.up(&d_n, n_vec, (size_t)m, st);
-  if (e == cudaSuccess) e = b.up(&d_lv, log_var, (size_t)m, st);
-  if (e == cudaSuccess) e = b.up(&d_pi, p_init, (size_t)nchain, st);
-  if (e == cudaSuccess) e = b.up(&d_sub, ind_sub, (size_t)m, st);
-  if (e == cudaSuccess) e = b.up(&d_rng, (const uint32_t *)rng_state, (size_t)6 * nchain, st);
+  b.up(&d_bh, beta_hat, (size_t)m, st);
+  b.up(&d_n, n_vec, (size_t)m, st);
+  b.up(&d_lv, log_var, (size_t)m, st);
+  b.up(&d_pi, p_init, (size_t)nchain, st);
+  b.up(&d_sub, ind_sub, (size_t)m, st);
+  b.up(&d_rng, (const uint32_t *)rng_state, (size_t)6 * nchain, st);
   double **outs[] = {&A.beta_est, &A.postp_est, &A.corr_est, &A.cb, &A.avg_b, &A.avg_p, &A.avg_bh, &A.abuf, &A.bbuf};
-  for (double **o : outs)
-    if (e == cudaSuccess) e = b.alloc(o, mc);
+  for (double **o : outs) b.alloc(o, mc);
   double **paths[] = {&A.path_p, &A.path_h2, &A.path_alpha};
-  for (double **o : paths)
-    if (e == cudaSuccess) e = b.alloc(o, tc);
-  if (e == cudaSuccess) e = b.alloc(&A.dot, (size_t)corr->ncol * nchain);
-  if (e == cudaSuccess) e = b.alloc(&A.causal, mc);
-  if (e == cudaSuccess && A.nrep) e = b.alloc(&A.sample, mc * A.nrep);
-  if (e == cudaSuccess) e = b.alloc(&A.ns, (size_t)nchain);
-  if (e == cudaSuccess && rng_out) e = b.alloc(&A.rng_out, (size_t)6 * nchain);
-  if (e != cudaSuccess) {
-    cudaGetLastError();
-    return fail(e == cudaErrorMemoryAllocation ? BSG_ERR_ALLOC : BSG_ERR_CUDA, "ldpred2_auto state (%s)", cudaGetErrorString(e));
-  }
+  for (double **o : paths) b.alloc(o, tc);
+  b.alloc(&A.dot, (size_t)corr->ncol * nchain);
+  b.alloc(&A.causal, mc);
+  if (A.nrep) b.alloc(&A.sample, mc * A.nrep);
+  b.alloc(&A.ns, (size_t)nchain);
+  if (rng_out) b.alloc(&A.rng_out, (size_t)6 * nchain);
+  BSG_TRY(b.status("ldpred2_auto state"));
   A.beta_hat = d_bh, A.n_vec = d_n, A.log_var = d_lv, A.p_init = d_pi, A.ind_sub = d_sub, A.rng = d_rng;
   k_ldpred2_auto<<<nchain, LT, 0, st>>>(corr->p, corr->rows, corr->first_i, corr->x, corr->ncol, A);
   count_launch();
@@ -1125,23 +1109,20 @@ int bsg_ldpred2_grid(bsg_sfbm *corr, const double *beta_hat, const double *n_vec
   double *d_bh = nullptr, *d_n = nullptr, *d_p = nullptr, *d_h2 = nullptr;
   int *d_sub = nullptr, *d_sp = nullptr;
   uint32_t *d_rng = nullptr;
-  cudaError_t e = b.up(&d_bh, beta_hat, (size_t)m, st);
-  if (e == cudaSuccess) e = b.up(&d_n, n_vec, (size_t)m, st);
-  if (e == cudaSuccess) e = b.up(&d_sub, ind_sub, (size_t)m, st);
-  if (e == cudaSuccess) e = b.up(&d_p, p, (size_t)npoint, st);
-  if (e == cudaSuccess) e = b.up(&d_h2, h2, (size_t)npoint, st);
-  if (e == cudaSuccess) e = b.up(&d_sp, sparse, (size_t)npoint, st);
-  if (e == cudaSuccess) e = b.up(&d_rng, (const uint32_t *)rng_state, (size_t)6 * npoint, st);
-  if (e == cudaSuccess) e = b.alloc(&A.beta_est, mp);
-  if (e == cudaSuccess) e = b.alloc(&A.cb, mp);
-  if (e == cudaSuccess) e = b.alloc(&A.avg, mp);
-  if (e == cudaSuccess) e = b.alloc(&A.dot, (size_t)corr->ncol * npoint);
-  if (e == cudaSuccess && sampling) e = b.alloc(&A.sample, smp);
-  if (e == cudaSuccess) e = b.alloc(&A.ns, (size_t)npoint);
-  if (e != cudaSuccess) {
-    cudaGetLastError();
-    return fail(e == cudaErrorMemoryAllocation ? BSG_ERR_ALLOC : BSG_ERR_CUDA, "ldpred2_grid state (%s)", cudaGetErrorString(e));
-  }
+  b.up(&d_bh, beta_hat, (size_t)m, st);
+  b.up(&d_n, n_vec, (size_t)m, st);
+  b.up(&d_sub, ind_sub, (size_t)m, st);
+  b.up(&d_p, p, (size_t)npoint, st);
+  b.up(&d_h2, h2, (size_t)npoint, st);
+  b.up(&d_sp, sparse, (size_t)npoint, st);
+  b.up(&d_rng, (const uint32_t *)rng_state, (size_t)6 * npoint, st);
+  b.alloc(&A.beta_est, mp);
+  b.alloc(&A.cb, mp);
+  b.alloc(&A.avg, mp);
+  b.alloc(&A.dot, (size_t)corr->ncol * npoint);
+  if (sampling) b.alloc(&A.sample, smp);
+  b.alloc(&A.ns, (size_t)npoint);
+  BSG_TRY(b.status("ldpred2_grid state"));
   A.beta_hat = d_bh, A.n_vec = d_n, A.p = d_p, A.h2 = d_h2, A.sparse = d_sp, A.ind_sub = d_sub, A.rng = d_rng;
   if (sampling)
     k_ldpred2_grid<true><<<npoint, LT, 0, st>>>(corr->p, corr->rows, corr->first_i, corr->x, corr->ncol, A);

@@ -480,24 +480,10 @@ __global__ void __launch_bounds__(ST) k_splreg(const FArgs<Src> a) {
 
 static thread_local double g_last_ms = 0, g_stage_ms = 0;
 
-struct Events {
-  cudaEvent_t ev[2] = {nullptr, nullptr};
-  ~Events() {
-    for (auto e : ev)
-      if (e) cudaEventDestroy(e);
-  }
-};
-
 static bool finite_all(const double *p, int64_t n) {
   for (int64_t i = 0; i < n; i++)
     if (!std::isfinite(p[i])) return false;
   return true;
-}
-
-static int scratch_fail(cudaError_t err) {
-  cudaGetLastError();
-  return fail(err == cudaErrorMemoryAllocation ? BSG_ERR_ALLOC : BSG_ERR_CUDA, "big_spLinReg scratch (%s)",
-              cudaGetErrorString(err));
 }
 
 // What an entry point hands the driver: the kernels' column source Src, the bounds n / m of ind_row / ind_col, the
@@ -516,22 +502,16 @@ struct BedOp {
   const char *bad_msg = "Column %d holds a missing value on a training row; impute it first (snp_fastImputeSimple).";
   size_t stage_bytes(int, int) const { return 0; }
   int stage(const std::vector<int> &row0, const std::vector<int> &col0, int nc, Bufs &b, Cols &cs) {
-    const bool dos = h->fbm_generic != 0;
-    if (dos) BSG_TRY(dosage_build(h));
-    int *d_rows, *d_cols, *d_lut = nullptr;
-    cudaError_t err = b.up(&d_rows, row0, s);
-    if (err == cudaSuccess) err = b.up(&d_cols, col0.data(), (size_t)nc, s);
-    if (dos) {
-      std::vector<int> tab(256);
-      for (int c = 0; c < 256; c++)
-        tab[c] = h->code256[c] != h->code256[c] ? -1 : (int)nearbyint(h->dos_scale * h->code256[c]);
-      if (err == cudaSuccess) err = b.up(&d_lut, tab, s);
-    }
-    if (err != cudaSuccess) return scratch_fail(err);
-    lut = d_lut;
-    cs.P = dos ? h->dosV : h->A;
-    cs.stride = dos ? h->dosStride : h->strideA;
-    cs.D = dos ? (double)h->dos_scale : 0.0;
+    Genotypes g;
+    BSG_TRY(genotypes(h, b, &g));
+    int *d_rows, *d_cols;
+    b.up(&d_rows, row0, s);
+    b.up(&d_cols, col0.data(), (size_t)nc, s);
+    BSG_TRY(b.status("big_spLinReg scratch"));
+    lut = g.lut;
+    cs.P = g.P;
+    cs.stride = g.stride;
+    cs.D = g.D;
     cs.rows = d_rows, cs.lines = d_cols;
     return BSG_OK;
   }
@@ -570,9 +550,9 @@ struct DenseOp {
     for (int c = 0; c < nc; c++) iota[c] = c;
     T *d_X;
     int *d_cols;
-    cudaError_t err = b.alloc(&d_X, (size_t)nr * nc);
-    if (err == cudaSuccess) err = b.up(&d_cols, iota, s);
-    if (err != cudaSuccess) return scratch_fail(err);
+    b.alloc(&d_X, (size_t)nr * nc);
+    b.up(&d_cols, iota, s);
+    BSG_TRY(b.status("big_spLinReg scratch"));
     bool contiguous = true;  // ind_row a run of consecutive rows: one copy per column
     for (int r = 1; r < nr && contiguous; r++) contiguous = row0[r] == row0[0] + r;
     const size_t colb = (size_t)nr * sizeof(T);
@@ -629,18 +609,9 @@ static int splreg_drive(Op &op, const int *ind_row, int nr, const int *ind_col, 
       !loss || !nnz || !npass)
     return fail(BSG_ERR_ARG, "null argument");
   const int n = op.n;
-  std::vector<int> row0(nr);
-  for (int r = 0; r < nr; r++) {
-    const int i = ind_row ? ind_row[r] : r + 1;
-    if (i < 1 || i > n) return fail(BSG_ERR_BOUNDS, "Tested subscript out of bounds (%d not in 1..%d).", i, n);
-    row0[r] = i - 1;
-  }
-  std::vector<int> col0(std::max(nc, 1));
-  for (int c = 0; c < nc; c++) {
-    const int j = ind_col ? ind_col[c] : c + 1;
-    if (j < 1 || j > op.m) return fail(BSG_ERR_BOUNDS, "Tested subscript out of bounds (%d not in 1..%d).", j, op.m);
-    col0[c] = j - 1;
-  }
+  std::vector<int> row0, col0;
+  BSG_TRY(host_index(ind_row, nr, n, "", row0));
+  BSG_TRY(host_index(ind_col, nc, op.m, "", col0));
   if (!finite_all(y, nr)) return fail(BSG_ERR_ARG, "'y.train' must be finite.");
   if (family == 1)
     for (int r = 0; r < nr; r++)
@@ -690,17 +661,14 @@ static int splreg_drive(Op &op, const int *ind_row, int nr, const int *ind_col, 
   g_stage_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
   double *d_cov = nullptr, *d_ctr, *d_sc;
   uint8_t *d_na;
-  cudaError_t err = cudaSuccess;
-  if (Kc > 0) err = b.up(&d_cov, covar, (size_t)nr * Kc, s);
-  if (err == cudaSuccess) err = b.alloc(&d_ctr, (size_t)Jall);
-  if (err == cudaSuccess) err = b.alloc(&d_sc, (size_t)Jall);
-  if (err == cudaSuccess) err = b.alloc(&d_na, (size_t)Jall);
-  if (err != cudaSuccess) return scratch_fail(err);
+  if (Kc > 0) b.up(&d_cov, covar, (size_t)nr * Kc, s);
+  b.alloc(&d_ctr, (size_t)Jall);
+  b.alloc(&d_sc, (size_t)Jall);
+  b.alloc(&d_na, (size_t)Jall);
+  BSG_TRY(b.status("big_spLinReg scratch"));
   cs.cov = d_cov, cs.nr = nr, cs.G = nc;
-  Events tm;
-  BSG_CUDA(cudaEventCreate(&tm.ev[0]));
-  BSG_CUDA(cudaEventCreate(&tm.ev[1]));
-  BSG_CUDA(cudaEventRecord(tm.ev[0], s));
+  CallTimer tm;
+  BSG_CUDA(tm.start(s));
   if (Jall > 0) {
     k_sp_stats<<<(Jall + ST / 32 - 1) / (ST / 32), ST, 0, s>>>(cs, Jall, op.raw, n, op.lut, d_ctr, d_sc, d_na);
     count_launch();
@@ -749,41 +717,41 @@ static int splreg_drive(Op &op, const int *ind_row, int nr, const int *ind_col, 
   std::vector<int> prow(pos.size());
   for (size_t i = 0; i < pos.size(); i++) prow[i] = row0[pos[i]];
   double *d_fc, *d_fis, *d_fpf, *d_y, *d_base, *d_al;
-  err = b.up(&d_lines, lines.data(), lines.size(), s);
-  if (err == cudaSuccess) err = b.up(&d_fc, fc, s);
-  if (err == cudaSuccess) err = b.up(&d_fis, fis, s);
-  if (err == cudaSuccess) err = b.up(&d_fpf, fpf, s);
-  if (err == cudaSuccess) err = b.up(&d_y, y, (size_t)nr, s);
-  if (err == cudaSuccess) err = b.up(&d_base, base ? base : zero.data(), (size_t)nr, s);
-  if (err == cudaSuccess) err = b.up(&d_al, alphas, (size_t)nalpha, s);
-  if (err == cudaSuccess) err = b.up(&d_pos, pos, s);
-  if (err == cudaSuccess) err = b.up(&d_prow, prow, s);
-  if (err == cudaSuccess) err = b.up(&d_ntr, ntr, s);
+  b.up(&d_lines, lines.data(), lines.size(), s);
+  b.up(&d_fc, fc, s);
+  b.up(&d_fis, fis, s);
+  b.up(&d_fpf, fpf, s);
+  b.up(&d_y, y, (size_t)nr, s);
+  b.up(&d_base, base ? base : zero.data(), (size_t)nr, s);
+  b.up(&d_al, alphas, (size_t)nalpha, s);
+  b.up(&d_pos, pos, s);
+  b.up(&d_prow, prow, s);
+  b.up(&d_ntr, ntr, s);
   double *d_r, *d_w = nullptr, *d_s = nullptr, *d_beta, *d_z, *d_v, *d_bb, *d_b0, *d_lam, *d_loss, *d_pb = nullptr,
          *d_pb0 = nullptr;
   uint8_t *d_flag;
   int *d_wl, *d_best, *d_len, *d_msg, *d_nnz, *d_np;
   const size_t FJ = (size_t)F * J, FL = (size_t)F * nlambda;
-  if (err == cudaSuccess) err = b.alloc(&d_r, (size_t)F * nr);
-  if (err == cudaSuccess && family == 1) err = b.alloc(&d_w, (size_t)F * nr);
-  if (err == cudaSuccess && family == 1) err = b.alloc(&d_s, (size_t)F * nr);
-  if (err == cudaSuccess) err = b.alloc(&d_beta, FJ);
-  if (err == cudaSuccess) err = b.alloc(&d_z, FJ);
-  if (err == cudaSuccess) err = b.alloc(&d_v, FJ);
-  if (err == cudaSuccess) err = b.alloc(&d_bb, FJ);
-  if (err == cudaSuccess) err = b.alloc(&d_flag, FJ * CS);
-  if (err == cudaSuccess) err = b.alloc(&d_wl, FJ * CS);
-  if (err == cudaSuccess) err = b.alloc(&d_b0, (size_t)F);
-  if (err == cudaSuccess) err = b.alloc(&d_best, (size_t)F);
-  if (err == cudaSuccess) err = b.alloc(&d_len, (size_t)F);
-  if (err == cudaSuccess) err = b.alloc(&d_msg, (size_t)F);
-  if (err == cudaSuccess) err = b.alloc(&d_lam, FL);
-  if (err == cudaSuccess) err = b.alloc(&d_loss, FL);
-  if (err == cudaSuccess) err = b.alloc(&d_nnz, FL);
-  if (err == cudaSuccess) err = b.alloc(&d_np, FL);
-  if (err == cudaSuccess && path_beta) err = b.alloc(&d_pb, FL * J);
-  if (err == cudaSuccess && path_b0) err = b.alloc(&d_pb0, FL);
-  if (err != cudaSuccess) return scratch_fail(err);
+  b.alloc(&d_r, (size_t)F * nr);
+  if (family == 1) b.alloc(&d_w, (size_t)F * nr);
+  if (family == 1) b.alloc(&d_s, (size_t)F * nr);
+  b.alloc(&d_beta, FJ);
+  b.alloc(&d_z, FJ);
+  b.alloc(&d_v, FJ);
+  b.alloc(&d_bb, FJ);
+  b.alloc(&d_flag, FJ * CS);
+  b.alloc(&d_wl, FJ * CS);
+  b.alloc(&d_b0, (size_t)F);
+  b.alloc(&d_best, (size_t)F);
+  b.alloc(&d_len, (size_t)F);
+  b.alloc(&d_msg, (size_t)F);
+  b.alloc(&d_lam, FL);
+  b.alloc(&d_loss, FL);
+  b.alloc(&d_nnz, FL);
+  b.alloc(&d_np, FL);
+  if (path_beta) b.alloc(&d_pb, FL * J);
+  if (path_b0) b.alloc(&d_pb0, FL);
+  BSG_TRY(b.status("big_spLinReg scratch"));
   BSG_CUDA(cudaMemsetAsync(d_bb, 0, FJ * sizeof(double), s));
   BSG_CUDA(cudaMemsetAsync(d_b0, 0, (size_t)F * sizeof(double), s));
   BSG_CUDA(cudaMemsetAsync(d_lam, 0, FL * sizeof(double), s));
@@ -814,7 +782,7 @@ static int splreg_drive(Op &op, const int *ind_row, int nr, const int *ind_col, 
   BSG_CUDA(cudaLaunchKernelEx(&cfg, k_splreg<typename Op::Src>, a));
   count_launch();
   BSG_CUDA(cudaGetLastError());
-  BSG_CUDA(cudaEventRecord(tm.ev[1], s));
+  BSG_CUDA(tm.stop(s));
   BSG_CUDA(cudaMemcpyAsync(beta, d_bb, FJ * sizeof(double), cudaMemcpyDeviceToHost, s));
   BSG_CUDA(cudaMemcpyAsync(intercept, d_b0, (size_t)F * sizeof(double), cudaMemcpyDeviceToHost, s));
   BSG_CUDA(cudaMemcpyAsync(best, d_best, (size_t)F * sizeof(int), cudaMemcpyDeviceToHost, s));
@@ -841,9 +809,7 @@ static int splreg_drive(Op &op, const int *ind_row, int nr, const int *ind_col, 
   };
   unpermute(beta, (size_t)F);
   if (path_beta) unpermute(path_beta, FL);
-  float ms = 0;
-  cudaEventElapsedTime(&ms, tm.ev[0], tm.ev[1]);
-  g_last_ms = ms;
+  g_last_ms = tm.ms();
   return BSG_OK;
 }
 
@@ -862,9 +828,7 @@ int bsg_splreg(bsg_bed *h, const int *ind_row, int nr, const int *ind_col, int n
                int *message, double *lambda, double *loss, int *nnz, int *npass, double *path_beta, double *path_b0) {
   using namespace splreg;
   if (!h) return fail(BSG_ERR_ARG, "null handle");
-  if (h->fbm_generic && !h->dos_scale)
-    return fail(BSG_ERR_TYPE, "big_spLinReg / big_spLogReg on the device need hard calls or dosages (codes multiples of "
-                              "1 / D); this FBM.code256 holds other values.");
+  BSG_TRY(genotypes_check(h, "big_spLinReg / big_spLogReg on the device need"));
   BSG_TRY(bind_device(h));
   BedOp op{h, h->n, h->m, h->stream, h->raw};
   return splreg_drive(op, ind_row, nr, ind_col, nc, family, y, covar, Kc, base, pf_X, pf_covar, alphas, nalpha,

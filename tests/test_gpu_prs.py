@@ -173,6 +173,9 @@ def test_abi_errors(example):
     assert L.bsg_prs_grid(f._h, pi(one), 1, 1, pi(one), pi(one), pd(b), None, pd(np.array([-1.0])), 1, pd(b), 1, optr) == 9
     assert L.bsg_prs_grid(f._h, pi(one), 1, 1, pi(one), pi(np.array([G.shape[1] + 1], np.int32)), pd(b), None, pd(b), 1,
                           pd(b), 1, optr) == 2
+    # a row out of range
+    assert L.bsg_prs_grid(f._h, pi(np.array([G.shape[0] + 1], np.int32)), 1, 1, pi(one), pi(one), pd(b), None, None, 1,
+                          None, 1, optr) == 2
     # a generic table (codes that are not multiples of 1 / D)
     code = np.full(256, np.nan)
     code[:201] = np.sqrt(np.arange(201))

@@ -251,5 +251,11 @@ def test_refusals(B, codes):
     yb[3] = np.nan
     with pytest.raises(B.BsgError):
         B.big_spLinReg(X, yb, ind_col=cols)
-    with pytest.raises(B.BsgError):
+    with pytest.raises(B.BsgError) as e:
         B.big_spLinReg(X, y, ind_col=[1, M + 1])
+    assert e.value.code == 2
+    code256 = np.full(256, np.nan)
+    code256[:3] = [0, 0.1234567, 2]  # not a dosage table: no scale D makes every code an integer byte
+    with pytest.raises(B.BsgError) as e:
+        B.big_spLinReg(B.Bed.from_fbm(codes, code256), y, ind_col=cols)
+    assert e.value.code == 10
